@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- snapshot-stream GiB/s of the peer-bootstrap hot path on B200.
+"""bench.py -- snapshot-stream GiB/s of the peer-bootstrap hot path on H100.
 
 Headline workload = BASELINE.json configs[2], the config its `metric` ("Fletcher-4+LZ4") is quoted
-on: a 64 GiB (logical) ZFS-send stream of LZ4-compressed 128 KiB records, mode RECOMPRESS
+on: a 32 GiB (logical) ZFS-send stream of LZ4-compressed 128 KiB records, mode RECOMPRESS
 (decode -> verify every stream checksum -> re-encode with the declared ZFS encoder -> re-stamp).
 One "step" = one full pass of the stage over that stream.  The metric counts INPUT STREAM bytes
 (SURVEY.md 8d: wire-format bytes, headers + compressed payloads, BEGIN...END) per second.
@@ -18,7 +18,14 @@ One "step" = one full pass of the stage over that stream.  The metric counts INP
             the oracle port of the same arithmetic on all host threads (oracle/mt.c), on a bounded
             sample of the same workload.  Reported, not the target.
 
-N > 1 (torchrun, one rank per GPU): STRONG scaling of the same 64 GiB stream, partitioned by record
+The stream is sized for one 80 GB H100: resident input (~13 GiB) + output (~32 GiB) + the codec
+scratch of two handles (16 GiB).
+
+`--dump-outputs DIR` writes, after the timed steps, what the last timed step computed (a seeded
+sample of the output stream, the output byte counts and the END checksum) as DIR/<name>.npy, so
+that two builds can be compared output for output on identical inputs.
+
+N > 1 (torchrun, one rank per GPU): STRONG scaling of the same stream, partitioned by record
 index into N contiguous shards; the only data-path exchange is the library-owned NCCL all-gather of
 the 40-byte shard aggregate plus the 32-byte output checksum hopping rank to rank
 (mtz_dev_finish_exchange).  Rank 0 then measures, in one process over all N GPUs, `e2e` and the
@@ -52,7 +59,7 @@ def parse_args():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="recompress", choices=["recompress", "verify"])
     ap.add_argument("--gib", type=float, default=0.0,
-                    help="workload size: logical GiB of the whole job (recompress, default 64) / "
+                    help="workload size: logical GiB of the whole job (recompress, default 32) / "
                          "stream GiB per GPU (verify, default 16)")
     ap.add_argument("--ref-gib", type=float, default=8.0,
                     help="CPU arms: GiB (logical for recompress) of the bounded sample each step processes")
@@ -62,7 +69,45 @@ def parse_args():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-reencode", action="store_true", help="skip the certificate-off resident leg (N=1)")
     ap.add_argument("--recsize", type=int, default=131072, help="DRR_WRITE logical size (dataset recordsize)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (float64, <= 64 MB)")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    return args
+
+
+DUMP_SAMPLE_BYTES = 4 << 20          # output-stream bytes sampled into the dump (32 MB as float64)
+
+
+def dump_outputs(d, arrays):
+    """arrays: name -> numpy array; written as float64 (every value here is an integer < 2^53)"""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(d, name + ".npy"), np.asarray(a, dtype=np.float64))
+
+
+def checksum_words(ck):
+    """a 4 x u64 checksum as 4 x [high 32, low 32] (exact in float64), zeros when absent"""
+    import numpy as np
+    ck = ck or (0, 0, 0, 0)
+    return np.array([[x >> 32, x & 0xffffffff] for x in ck], dtype=np.float64)
+
+
+def dev_equal(a, b, chunk=1 << 30):
+    """torch.equal of two device byte tensors, a GiB at a time: a whole-stream comparison would
+    need a temporary as large as the stream, which an 80 GB card holding it twice cannot spare"""
+    import torch
+    return a.numel() == b.numel() and all(bool(torch.equal(a[o:o + chunk], b[o:o + chunk]))
+                                          for o in range(0, a.numel(), chunk))
+
+
+def sample_positions(total, n, seed=0x4D545A):
+    """n sorted byte positions in [0, total), the same for the same total"""
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    return np.sort(rng.integers(0, total, size=min(n, total), dtype=np.int64)) if total > 0 else np.zeros(0, np.int64)
 
 
 class ClockSampler(object):
@@ -147,7 +192,7 @@ def load_peaks():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(peaks["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (a STREAM copy, read+write)"
     except Exception:
-        return 6650.0, "fallback 6650 GB/s (B200_PROFILING.md)"
+        return 3350.0, "fallback 3350 GB/s (H100 SXM data-sheet HBM3 bandwidth, not a measured copy)"
 
 
 # ------------------------------------------------------------------ CPU legs (oracle port) --
@@ -250,7 +295,7 @@ def run_reference(args):
                   "(oracle/mt.c)" % (s.size / GIB, SIMD_NAME.get(O.simd_lanes(), "scalar")))
         dtype = "u32->u64 (mod 2^64)"
     else:
-        gib = args.gib or 64.0
+        gib = args.gib or 32.0
         src, logical, _ = make_lz4_stream(O, min(args.ref_gib, gib), nthreads, pinned=False)
         out = np.empty(src.size + (1 << 20), dtype=np.uint8)
         for _ in range(max(1, min(args.warmup, 2))):
@@ -288,12 +333,15 @@ _PUMP = None
 
 def ring_pump():
     """tools/libringpump.so: native producers for the ring API (bench infrastructure, built by
-    __graft_entry__.build(); rebuilt here if it did not travel)."""
+    __graft_entry__.build(); rebuilt into a temporary directory if it is missing -- the tree may be
+    read-only)."""
     global _PUMP
     if _PUMP is None:
         import ctypes as C
+        import tempfile
         so = os.path.join(ROOT, "tools", "libringpump.so")
         if not os.path.exists(so):
+            so = os.path.join(tempfile.mkdtemp(prefix="mtz_bench_"), "libringpump.so")
             subprocess.check_call(["gcc", "-O2", "-shared", "-fPIC", "-pthread", "-o", so,
                                    os.path.join(ROOT, "tools", "ringpump.c")])
         P = C.CDLL(so)
@@ -407,12 +455,13 @@ def ring_run(g, src, peers=(0,), producer="write", nthreads=4, chunk=64 << 20, l
 
 
 # -------------------------------------------------------------------------------- our arm --
-def run_verify_resident(args, O, local, steps, warm, peak):
+def run_verify_resident(args, O, local, steps, warm, peak, dump=None):
     """configs[1] on one GPU: 16 GiB uncompressed stream resident in HBM; GPU parse + K1 + scan per
-    step (round 1's headline, kept as a workload)."""
+    step (round 1's headline, kept as a workload).  `dump`: directory for the last step's outputs."""
     import numpy as np
     import torch
     from manatee_b200 import GpuSnapshotStage, PinnedBuffer, index_host
+    from manatee_b200.stage import REC_DTYPE
     gib = args.verify_gib if args.workload != "verify" else (args.gib or 16.0)
     nthreads = host_threads()
     nwrites = max(1, int(gib * GIB) // REC_BYTES)
@@ -440,13 +489,21 @@ def run_verify_resident(args, O, local, steps, warm, peak):
         torch.cuda.synchronize()
         e0.record(st)
         for _ in range(steps):
-            step()
+            last = step()
         e1.record(st)
         torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / steps
         s1 = g.stats()
         k1_ms = (s1["k1_ms"] - s0["k1_ms"]) / max(1, s1["k1_launches"] - s0["k1_launches"])
         end_ck = g.end_checksum()
+        if dump:
+            # the last step's record table (mtz_dev_index; the first 1 Mi records) and verdict
+            n_dump = min(len(recs), 1 << 20)
+            t = d_recs[:n_dump * 32].cpu().numpy().view(REC_DTYPE)
+            dump_outputs(dump, {"verify_record_table": np.stack([t["off"], t["payload"], t["type"], t["lsize"]], 1),
+                                "verify_output_bytes": [last[0]],
+                                "verify_input_checksum": checksum_words(last[1]),
+                                "verify_end_checksum": checksum_words(end_ck)})
         res.update({"value": round(s.size / GIB / (ms / 1e3), 3), "unit": "GiB/s", "ms_per_step": round(ms, 4),
                     "steps": steps, "gpu_launches": int((s1["kernel_launches"] - s0["kernel_launches"]) // steps),
                     "config": verify_config(gib),
@@ -454,7 +511,8 @@ def run_verify_resident(args, O, local, steps, warm, peak):
                                  "achieved": round(s.size / (k1_ms / 1e3) / 1e9, 1), "peak": peak, "unit": "GB/s",
                                  "frac": round(s.size / (k1_ms / 1e3) / 1e9 / peak, 4), "traffic": None,
                                  "algorithmic_bytes_per_launch": float(s.size), "k1_ms": round(k1_ms, 4),
-                                 "note": "K1 only reads; the peak is a copy (read+write), so ~1.0 is the roof"}})
+                                 "peak_source": load_peaks()[1],
+                                 "note": "K1 only reads the stream; the peak is the HBM figure peak_source names"}})
     del d_stream, d_recs
     torch.cuda.empty_cache()
     if not args.no_e2e:
@@ -517,7 +575,7 @@ def run_ours(args):
                              "line is the recompress workload")
         clocks = ClockSampler(local); clocks.start()
         t0 = time.time()
-        r = run_verify_resident(args, O, local, args.steps, args.warmup, peak)
+        r = run_verify_resident(args, O, local, args.steps, args.warmup, peak, dump=args.dump_outputs)
         clk = clocks.stop(t0, time.time())
         line = {"metric": "snapshot_stream_gibs", "value": r["value"], "unit": "GiB/s", "n_gpus": 1,
                 "steps": args.steps, "warmup": args.warmup, "ms_per_step": r["ms_per_step"],
@@ -530,7 +588,7 @@ def run_ours(args):
         return 0
 
     # ------------------------------------------------------------------ the stream (rank 0 makes it)
-    total_gib = args.gib or 64.0
+    total_gib = args.gib or 32.0
     shm = "/dev/shm/mtz_bench_%s.bin" % os.environ.get("MASTER_PORT", str(os.getpid()))
     src = pin_in = None
     meta = [None]
@@ -630,7 +688,7 @@ def run_ours(args):
         obs = step()
     # size-independent parity at full size: the input was produced by the declared encoder, so
     # RECOMPRESS must reproduce every chunk bit for bit (idempotence), re-stamped checksums included
-    ok_all = all(ob == c["bytes"] and bool(torch.equal(c["d_out"][:ob], c["d_in"][:c["bytes"]]))
+    ok_all = all(ob == c["bytes"] and dev_equal(c["d_out"][:ob], c["d_in"][:c["bytes"]])
                  for ob, c in zip(obs, chunks))
     same = torch.tensor([1 if ok_all else 0], device="cuda")
     if world > 1:
@@ -642,9 +700,24 @@ def run_ours(args):
     t_wall0 = time.time()
     e0.record(sts[0])
     for _ in range(args.steps):
-        step()
+        obs = step()
     e1.record(sts[(CH - 1) % len(hs)])          # the stream of the last chunk; every finish has synchronised
     torch.cuda.synchronize()
+    if args.dump_outputs:
+        # this rank's output of the last timed step: its chunks' output bytes (in chunk order) at
+        # seeded positions that depend only on their total, every chunk's output byte count and
+        # the END checksum
+        tot = sum(obs)
+        pos = torch.from_numpy(sample_positions(tot, DUMP_SAMPLE_BYTES)).cuda()
+        bnd = torch.tensor(np.cumsum([0] + list(obs)), device="cuda")
+        sample = torch.empty(pos.numel(), dtype=torch.uint8, device="cuda")
+        for k, c in enumerate(chunks):
+            sel = (pos >= bnd[k]) & (pos < bnd[k + 1])
+            sample[sel] = c["d_out"][pos[sel] - bnd[k]]
+        sfx = "" if world == 1 else "_rank%d" % rank
+        dump_outputs(args.dump_outputs, {"recompress_output_sample" + sfx: sample.cpu().numpy(),
+                                         "recompress_output_bytes" + sfx: np.array(obs),
+                                         "recompress_end_checksum" + sfx: checksum_words(end_ck[0])})
     if world > 1:
         dist.barrier()
     t = torch.tensor([e0.elapsed_time(e1)], dtype=torch.float64, device="cuda")
@@ -672,7 +745,7 @@ def run_ours(args):
                                   c["d_out"].data_ptr(), c["d_out"].numel(), cuda_stream=sts[0].cuda_stream)
                     return g2.dev_finish()[0]
                 ob2 = one()
-                ok2 = (ob2 == c["bytes"] and bool(torch.equal(c["d_out"][:ob2], c["d_in"][:c["bytes"]])))
+                ok2 = (ob2 == c["bytes"] and dev_equal(c["d_out"][:ob2], c["d_in"][:c["bytes"]]))
                 r0 = torch.cuda.Event(enable_timing=True); r1 = torch.cuda.Event(enable_timing=True)
                 torch.cuda.synchronize(); r0.record(sts[0])
                 kk = max(1, min(3, args.steps))
@@ -810,12 +883,6 @@ def run_ours(args):
         certified = n_enc > 0 and n_cert >= 0.5 * n_enc
         kname = "k3c_lz4_certify" if certified else "k3_lz4_encode"
         traffic = None
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles",
-                                             "r2_k3c_traffic.json" if certified else "r2_k3_traffic.json")))
-            traffic = tj.get("dram_bytes_per_algorithmic_byte") * alg / max(1.0, k3_launches)
-        except Exception:
-            pass
         cfg = recompress_config(total_gib)            # identical on both arms (the driver compares them)
         detail = {"records": int(len(recs_all)), "write_records": nwrites_total,
                   "stream_gib": round(total_bytes / GIB, 3), "logical_gib": round(logical / GIB, 3),
@@ -829,7 +896,7 @@ def run_ours(args):
                   "partition": ("record-index: %d chunks of whole records taken round-robin by %d ranks; per chunk a "
                                 "40-B aggregate all-gather + the 32-B output checksum travelling the ring, "
                                 "library-owned NCCL" % (4 * world, world)) if world > 1 else "single GPU",
-                  "l2": "inputs_exceed_l2 (%.1f GiB per GPU >> 126 MB)" % (total_bytes / world / GIB)}
+                  "l2": "inputs_exceed_l2 (%.1f GiB per GPU >> 50 MB)" % (total_bytes / world / GIB)}
         line = {
             "metric": "snapshot_stream_gibs", "value": round(value, 3), "unit": "GiB/s",
             "n_gpus": world, "steps": args.steps, "warmup": args.warmup,

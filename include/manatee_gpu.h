@@ -1,5 +1,5 @@
 /*
- * manatee_gpu.h -- C ABI of libmanatee_gpu.so, the B200 snapshot-stream stage.
+ * manatee_gpu.h -- C ABI of libmanatee_gpu.so, the H100 snapshot-stream stage.
  *
  * This is the drop-in boundary for the one bulk-data path of
  * TritonDataCenter/manatee: the ZFS-send byte stream that the sender pumps
@@ -42,7 +42,7 @@ extern "C" {
 #define MTZ_ENOSPC   -7   /* output capacity exceeded */
 #define MTZ_ENOMEM   -8
 #define MTZ_EOF      -9   /* consumer: stream finished and fully drained */
-#define MTZ_ENOGPU  -10   /* no usable sm_100 device: there is NO CPU fallback */
+#define MTZ_ENOGPU  -10   /* no usable sm_90 device: there is NO CPU fallback */
 #define MTZ_ECANCELED -11 /* mtz_cancel(): the pipe was torn down from outside */
 
 /* ---- stage modes ---- */
@@ -135,7 +135,7 @@ typedef struct mtz_job {
  * (spawn at lib/zfsClient.js:793); opened when the child is spawned, closed when
  * the pipe ends or fails. */
 int32_t     mtz_abi_version(void);
-int32_t     mtz_device_count(void);                 /* sm_100 devices visible, <0 on error */
+int32_t     mtz_device_count(void);                 /* sm_90 devices visible, <0 on error */
 int32_t     mtz_open(const mtz_config *cfg, mtz_handle **out);
 int32_t     mtz_close(mtz_handle *h);
 const char *mtz_last_error(mtz_handle *h);          /* h may be NULL: last open() error */

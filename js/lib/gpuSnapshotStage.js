@@ -7,7 +7,7 @@
  *
  * All work happens in libmanatee_gpu.so on the GPU; this file only moves Buffers
  * between Node's stream machinery and the library's pinned rings.  There is no
- * JS/CPU fallback: if the addon cannot be loaded or no B200 is present, creating
+ * JS/CPU fallback: if the addon cannot be loaded or no H100 is present, creating
  * a stage throws, and the caller's `gpu.mode` must be 'off' to get the legacy
  * identity pipe.
  *

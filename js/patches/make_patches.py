@@ -7,8 +7,9 @@ Each edit is an (anchor text -> replacement) pair applied to the maintainer's fi
 script fails loudly if an anchor is missing or ambiguous (i.e. if upstream moved), then
 writes `diff -u` output with a/ b/ prefixes, so that in a manatee checkout
     patch -p1 < js/patches/backupSender.js.patch
-applies as is.  tests/test_js_patches.py re-applies them to a scratch copy whenever the
-reference tree is available.  Only the three edited files are read; nothing of the
+applies as is.  tests/test_js_patches.py checks them against tests/golden/js_patch_targets.json
+(line digests of the upstream files; regenerate it with tests/golden/make_js_patch_golden.py
+after regenerating the patches).  Only the three edited files are read; nothing of the
 reference is stored here beyond the context lines a unified diff carries.
 
 What the edits do (INTEGRATION.md):

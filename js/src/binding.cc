@@ -5,7 +5,7 @@
 // (`node --version`: not found).  The test-suite compiles this very file against a stub of
 // the N-API declarations (tests/stubs/node_api.h), links it with a miniature in-process
 // N-API (tests/stubs/napi_mock.cc) and executes it through tests/stubs/napi_harness.cc --
-// on the CPU with an in-memory stand-in of the library, on a B200 with the real one
+// on the CPU with an in-memory stand-in of the library, on an H100 with the real one
 // (tests/test_zz_napi_harness.py).
 //
 // JS surface (used by js/lib/gpuSnapshotStage.js):

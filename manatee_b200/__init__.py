@@ -1,4 +1,4 @@
-"""manatee_b200 -- B200-native snapshot-stream stage for TritonDataCenter/manatee's
+"""manatee_b200 -- H100-native snapshot-stream stage for TritonDataCenter/manatee's
 peer-bootstrap pipeline (lib/backupSender.js -> lib/backupServer.js ->
 lib/zfsClient.js).  See DESIGN.md; the product is ``libmanatee_gpu.so`` (C ABI in
 ``include/manatee_gpu.h``), this package is its host-side mirror."""

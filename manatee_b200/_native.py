@@ -8,7 +8,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# MTZ_SO: load another build of the SAME library (kernel A/B experiments, tools/gpu/); default in-tree
+# MTZ_SO: load another build of the SAME library (kernel A/B experiments); default in-tree
 SO_PATH = os.environ.get("MTZ_SO") or os.path.join(_HERE, "libmanatee_gpu.so")
 
 OK, EINVAL, EAGAIN, ECUDA, EFORMAT, ECKSUM, ECODEC, ENOSPC, ENOMEM, EOF, ENOGPU, ECANCELED = \

@@ -1,4 +1,4 @@
-// fletcher.cuh -- K1: Fletcher-4 partial sums on sm_100a (integer, HBM-bound).
+// fletcher.cuh -- K1: Fletcher-4 partial sums on sm_90a (integer, HBM-bound).
 //
 // The arithmetic replaced here runs today inside the `zfs send` / `zfs recv`
 // children that the reference spawns (lib/backupSender.js:177,
@@ -95,7 +95,7 @@ __host__ __device__ __forceinline__ Ck4 fold_cksum_words(Ck4 s, const Ck4 &v)
 #ifdef __CUDACC__
 
 #ifndef K1_UNROLL
-#define K1_UNROLL 12          // LDG.128 in flight per lane (profiles/r1_verify_k1.md)
+#define K1_UNROLL 12          // LDG.128 in flight per lane
 #endif
 
 __device__ __forceinline__ uint4 ldg_stream(const uint4 *p)

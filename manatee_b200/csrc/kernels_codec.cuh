@@ -274,8 +274,8 @@ k_assemble(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs, u
 // exchange the new value by shuffle.  BEGIN records (checksum field is data, running
 // value restarts), END records (the running value is also written into the payload-less
 // END header, which changes that header's sums) and the batch edges take the generic
-// path.  Round 1's one-lane recurrence cost 358 ns per record (5.9 ms per 16 384
-// records); see profiles/r2_stamp_chain.md for this one.
+// path.  This replaced a one-lane recurrence that walked every record through the full
+// Fletcher update.
 // Folded once more: x.a .. x.d ARE the halves (x_i = w_2i + 2^32 w_2i+1), so the apply() part
 // multiplies the same eight words -- component j of x_{r+1} is ONE linear form of w_0..w_7 plus a
 // constant, with 64-bit weights  C_k = T_j(n2+8-k) + E_j,i  (k = 2i)  or  + (E_j,i << 32)  (k = 2i+1),
@@ -395,9 +395,8 @@ __device__ __forceinline__ Ck4 stamp_leave(const Ck4 &x, const RecSums *__restri
 #define STAMP_THREADS 128
 #define STAMP_LOADERS (STAMP_THREADS / 32 - 1)
 // warp 0 walks the chain; warps 1..3 stage the next STAMP_GROUP transitions (12.8 KB) into shared
-// memory.  One loader warp with one load in flight per lane took ~12 000 cycles per group, four
-// times what the chain needs for it (profiles/r2_stamp_chain.md): three warps, four loads in
-// flight per lane
+// memory.  One loader warp with one load in flight per lane could not keep up with the chain:
+// three warps, four loads in flight per lane
 __global__ void __launch_bounds__(STAMP_THREADS)
 k_stamp_chain(uint8_t *__restrict__ d_out, const mtz_rec *__restrict__ out_recs,
     const RecSums *__restrict__ osums, const StampStep *__restrict__ steps, uint32_t n,

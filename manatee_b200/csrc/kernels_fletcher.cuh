@@ -54,8 +54,7 @@ __device__ __forceinline__ Ck4 load_ck(const uint8_t *p)   // 8-byte aligned
 // One WARP per record (grid-stride).  A 128 KiB record is 257 rows of 512 B:
 // the warp streams them with K1_UNROLL (12) LDG.128 in flight per lane, so the
 // per-call basis conversion and the warp reduction are paid once per record.
-// Measured sweep on B200 (profiles/r1_verify_k1.md): 4 CTAs/SM x 12 loads
-// (126 regs) 2.53 ms per 16 GiB > 5 x 8 (96 regs) 2.84 ms > 6 x 8 (spills) 2.66 ms.
+// 4 CTAs/SM x 12 loads in flight fit 126 registers without spills.
 // body_from = 280 (VERIFY: checksum field + payload) or 312 (payload only).
 __global__ void __launch_bounds__(K1_THREADS, K1_MINBLOCKS)
 k1_record_sums(const uint8_t *__restrict__ base, const mtz_rec *__restrict__ recs,

@@ -1,4 +1,4 @@
-// kernels_lz4.cuh -- K2 (ZFS-LZ4 decode) and K3 (ZFS-LZ4 encode), sm_100a.
+// kernels_lz4.cuh -- K2 (ZFS-LZ4 decode) and K3 (ZFS-LZ4 encode), sm_90a.
 //
 // Byte/integer work, no tensor cores.  The codec these kernels restate runs
 // today inside the `zfs` children the reference spawns (`zfs send` at
@@ -250,8 +250,8 @@ __device__ __forceinline__ uint32_t put_len_ext(uint8_t *dst, uint32_t op, uint3
 
 // ---------------------------------------------------------------------------
 // The matcher.  One LZ4 sequence costs three dependent global round trips (an
-// earlier version needed seven; profiles/r1_k3_encode.md: K3 is bound by latency
-// chains at <= 24 warps/SM, not by bandwidth):
+// earlier version needed seven; K3 is bound by latency chains at <= 24 warps/SM,
+// not by bandwidth):
 //   trip A  candidate gather of a search round (positions come preloaded)
 //   trip B  catch-up bytes + first 32 literals + first match-extension round
 //   trip C  follow-on probe + its extension round + next search round's positions
@@ -327,8 +327,8 @@ __device__ __forceinline__ uint32_t warp_lz4_encode3(const uint8_t *__restrict__
 					h = (v * 2654435761u) >> (32 - LOG);
 				}
 				// Do two lanes of this round hash to the same slot?  __match_any_sync answers
-				// that but costs ~365 cycles on B200 when all 32 values differ (the common
-				// case; tools/micro/match_any.cu).  Cheaper: every lane already holds its
+				// that but costs hundreds of cycles when all 32 values differ (the common
+				// case; tools/micro/match_any.cu measures it).  Cheaper: every lane already holds its
 				// slot's value, so mark the slots with lane ids (~100 cycles) and look back.
 				uint32_t oldv = 0;
 				if (valid) oldv = tab.get(h);
@@ -570,8 +570,8 @@ __device__ __forceinline__ uint32_t warp_zfs_lz4_compress(const uint8_t *__restr
 // RECOMPRESS re-encodes what it has just decoded.  When the incoming block already IS what
 // lz4_encode (oracle/lz4_zfs.c:85-208) would emit for those bytes -- every block a `zfs send -c` of an
 // lz4 dataset carries, if the declared encoder is ZFS's -- the answer is the input, and PROVING that
-// is far cheaper than recomputing it: the serial matcher is a chain of ~5000 dependent cycles per
-// sequence (profiles/r2_k3_encode.md) because every decision waits for a gather from the source; a
+// is far cheaper than recomputing it: the serial matcher is a chain of thousands of dependent cycles
+// per sequence because every decision waits for a gather from the source; a
 // replay that is TOLD the parse (K2's sequence table) knows where the hits must be and only has to
 // keep the hash table honest.
 //

@@ -3,7 +3,7 @@
 // Replaces the data path of the reference's two pipes,
 //   zfsSend.stdout.pipe(socket)      lib/backupSender.js:179
 //   socket.pipe(zfsRecv.stdin)       lib/zfsClient.js:826
-// with: pinned host ring -> cudaMemcpyAsync -> HBM -> sm_100a kernels
+// with: pinned host ring -> cudaMemcpyAsync -> HBM -> sm_90a kernels
 // (Fletcher-4 verify / LZ4 decode / LZ4 encode / re-stamp) -> pinned ring.
 // There is NO CPU fallback: without a usable device mtz_open fails MTZ_ENOGPU.
 #include <cstdarg>
@@ -75,7 +75,7 @@ const char *mtz_strerror(int32_t code)
 	case MTZ_ENOSPC: return "output capacity exceeded";
 	case MTZ_ENOMEM: return "out of memory";
 	case MTZ_EOF: return "end of stream";
-	case MTZ_ENOGPU: return "no sm_100 GPU (no CPU fallback exists)";
+	case MTZ_ENOGPU: return "no sm_90 GPU (no CPU fallback exists)";
 	default: return "unknown error";
 	}
 }
@@ -96,7 +96,7 @@ int32_t mtz_device_count(void)
 	int ok = 0;
 	for (int i = 0; i < n; i++) {
 		cudaDeviceProp p;
-		if (cudaGetDeviceProperties(&p, i) == cudaSuccess && p.major == 10) ok++;
+		if (cudaGetDeviceProperties(&p, i) == cudaSuccess && p.major == 9 && p.minor == 0) ok++;
 	}
 	return ok;
 }
@@ -176,10 +176,9 @@ int32_t mtz_index_host(const void *buf, size_t n, mtz_rec *recs, size_t cap,
 // machine for tens of milliseconds per launch; with priorities on, its streams get the LEAST
 // priority and every other library stream the GREATEST, so that short kernels (plan, decode of the
 // next sub-batch, assemble, the stamp chain, the NCCL broadcast) are placed the moment an encoder
-// CTA retires.  Measured neutral to -1 % on one GPU and neutral for the fan-out on two
-// (profiles/r2_stream_priorities.md): the encoder is throughput-bound, whatever runs beside it
-// takes its issue slots either way.  What did help a little (+1-2 %) is launching K2/K3 as many
-// short-lived CTAs rather than one persistent wave (lz4_grid), which is the default.
+// CTA retires.  The encoder is throughput-bound, so whatever runs beside it takes its issue slots
+// either way; launching K2/K3 as many short-lived CTAs rather than one persistent wave (lz4_grid)
+// is the default.
 static bool stream_priorities()
 {
 	static const bool on = [] { const char *e = getenv("MTZ_STREAM_PRIORITIES"); return e != nullptr && atoi(e) != 0; }();
@@ -287,8 +286,8 @@ int32_t mtz_open(const mtz_config *cfg, mtz_handle **out)
 			return fail(nullptr, MTZ_EINVAL, "device %d out of range (%d visible)", d, ndev);
 		for (uint32_t k = 0; k < i; k++)
 			if (full.devices[k] == d) return fail(nullptr, MTZ_EINVAL, "device %d listed twice", d);
-		if (cudaGetDeviceProperties(&props[i], d) != cudaSuccess || props[i].major != 10)
-			return fail(nullptr, MTZ_ENOGPU, "device %d is sm_%d%d; this library is built for sm_100a only",
+		if (cudaGetDeviceProperties(&props[i], d) != cudaSuccess || props[i].major != 9 || props[i].minor != 0)
+			return fail(nullptr, MTZ_ENOGPU, "device %d is sm_%d%d; this library is built for sm_90a only",
 			    d, props[i].major, props[i].minor);
 	}
 	if (full.n_devices > 1 && (full.flags & MTZ_FLAG_DEFER_VERIFY))
@@ -1393,8 +1392,8 @@ int32_t mtz_process_host(mtz_handle *h, const void *in, size_t n, void *out, siz
 	// Output order == submission order.  Batches are retired (verdict folded in, output copy ISSUED)
 	// in order as soon as they are done -- looked at every iteration, not only when their slot
 	// comes round again: on a device group several GPUs' output copies then overlap on their own
-	// PCIe links instead of queueing behind one host wait per batch (43 -> ... GiB/s e2e at 4 GPUs,
-	// profiles/r2_scaling.md).  A slot is reused once its batch is retired and its copy has landed.
+	// PCIe links instead of queueing behind one host wait per batch.  A slot is reused once its
+	// batch is retired and its copy has landed.
 	const size_t NS = h->slots.size();
 	uint64_t nr = 0;                                  // batches retired so far
 	auto retire_next = [&](bool block) -> int32_t {   // 1 = the oldest batch is still running
@@ -1534,7 +1533,7 @@ static int32_t k3_set_attributes(mtz_handle *h)
 	MTZ_CU(h, cudaFuncSetAttribute(k3c_lz4_certify<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
 	    (int)((size_t)K3_WARPS * LZ4_TAB_BIG_WORDS * 4)));
 	{
-		// experiments: a smaller carve-out trades certificate warps per SM for L1 (profiles/r2_k3c_certify.md)
+		// experiments: a smaller carve-out trades certificate warps per SM for L1
 		const char *c = getenv("MTZ_K3C_CARVEOUT");
 		if (c != nullptr && atoi(c) > 0) {
 			MTZ_CU(h, cudaFuncSetAttribute(k3c_lz4_certify<true>, cudaFuncAttributePreferredSharedMemoryCarveout, atoi(c)));
@@ -1542,8 +1541,8 @@ static int32_t k3_set_attributes(mtz_handle *h)
 		}
 	}
 	// all of the unified L1/shared array as shared memory: K3 is bound by records in
-	// flight (24 tables of 8.5 KiB per SM), measured 62 vs 46 GiB/s at a 75 % carve-out
-	// (profiles/r1_k3_encode.md).  MTZ_K3_CARVEOUT overrides for experiments.
+	// flight (24 tables of 8.5 KiB per SM, which a 75 % carve-out cannot hold).
+	// MTZ_K3_CARVEOUT overrides for experiments.
 	const char *e = getenv("MTZ_K3_CARVEOUT");
 	const int pct = e ? atoi(e) : 100;
 	MTZ_CU(h, cudaFuncSetAttribute(k3_lz4_encode<true>, cudaFuncAttributePreferredSharedMemoryCarveout, pct));

@@ -8,7 +8,7 @@
 //     instance (CTAs of a launch run one after the other; a cooperative launch is emulated
 //     with a single CTA), global memory is ordinary memory.
 // This is test infrastructure only: nothing under tests/ is part of the product, which has no
-// CPU path (mtz_open fails with MTZ_ENOGPU without an sm_100 device).
+// CPU path (mtz_open fails with MTZ_ENOGPU without an sm_90 device).
 #pragma once
 #include <stdint.h>
 #include <stddef.h>

@@ -169,7 +169,7 @@ static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int)
 {
 	memset(p, 0, sizeof *p);
 	strcpy(p->name, "SIMT emulator (tests/emul)");
-	p->major = 10; p->minor = 0;
+	p->major = 9; p->minor = 0;
 	p->multiProcessorCount = 2;                 // small grids: the emulator runs CTAs one by one
 	p->totalGlobalMem = (size_t)8 << 30;
 	return cudaSuccess;

@@ -4,7 +4,7 @@
 //   * on the CPU, against tests/stubs/mtz_mock.cc (an in-memory stand-in for the library),
 //     to check the binding's own logic: argument marshalling, error throwing, the
 //     eventfd -> poll thread -> threadsafe-function wake-up path, external ArrayBuffers;
-//   * on a B200, against the real libmanatee_gpu.so: the same exported functions the JS
+//   * on an H100, against the real libmanatee_gpu.so: the same exported functions the JS
 //     Transform calls, driven in the same order, moving a real stream through the GPU.
 // What it does not cover is V8 itself and js/lib/gpuSnapshotStage.js.
 #include "node_api.h"

@@ -36,7 +36,7 @@ def test_error_strings_and_null_handles(native):
 
 
 def test_open_without_gpu_fails_loudly(native):
-    """No silent CPU fallback: on a box without a B200 mtz_open returns MTZ_ENOGPU."""
+    """No silent CPU fallback: on a box without an H100 mtz_open returns MTZ_ENOGPU."""
     import ctypes as C
     import torch
     from manatee_b200 import _native as N

@@ -4,7 +4,7 @@ compiled by g++ against tests/emul/cuda_runtime.h -- a stub that maps the warp i
 (warp_lz4_encode3 in all three table flavours, warp_zfs_lz4_compress, warp_lz4_decode,
 warp_fletcher / group_fletcher) are fuzzed against the oracle, inside guard-page buffers so an
 out-of-bounds access is a crash.  Far more inputs than the GPU suite can afford, no GPU needed;
-it is also how a kernel change can be checked for bit-exactness before it ever sees a B200.
+it is also how a kernel change can be checked for bit-exactness before it ever sees an H100.
 Test infrastructure only: the product has no CPU path."""
 import ctypes as C
 import os

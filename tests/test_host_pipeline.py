@@ -310,7 +310,7 @@ def _coalesced(fakezfs, tmp_path, sender_gpu, recv_gpu):
 class _IdentityStageDouble(object):
     """TEST DOUBLE with GpuSnapshotStage's streaming surface (write/flush/read/stats/close).
     It only lets the CPU suite walk the host threading around a stage (drain threads, job
-    fields, negotiation); the product has no such thing -- the real stage needs a B200."""
+    fields, negotiation); the product has no such thing -- the real stage needs an H100."""
     made = []
 
     def __init__(self, mode="verify", **kw):

@@ -7,7 +7,7 @@ every wake-up, stats, endChecksum, unwatch, close).
         marshalling, the eventfd -> poll thread -> threadsafe-function wake-up path, external
         ArrayBuffers, 64-bit BigInts, thrown errors carrying MTZ_E* codes and mtz_last_error;
         and against the REAL libmanatee_gpu.so, where open() must throw MTZ_ENOGPU here.
-  GPU:  linked against the real library: a stream goes through the binding and the B200 and
+  GPU:  linked against the real library: a stream goes through the binding and the H100 and
         comes back verified / compressed exactly as the oracle says.
 (The file sorts last on purpose: it is the newest test of the suite.)"""
 import json

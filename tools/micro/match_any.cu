@@ -1,4 +1,4 @@
-// microbenchmark: latency of __match_any_sync / ballot / shfl / smem atomics on sm_100a
+// microbenchmark: latency of __match_any_sync / ballot / shfl / smem atomics on sm_90a
 #include <cstdio>
 #include <cuda_runtime.h>
 __global__ void k(unsigned *out, long long *cyc, int mode)

@@ -1,4 +1,4 @@
-"""Summarise an .ncu-rep (raw page) + a launch-list csv into profiles/*.md|json."""
+"""Summarise an .ncu-rep (raw page) + a launch-list csv into markdown / json."""
 import csv, json, subprocess, sys
 from collections import defaultdict
 
