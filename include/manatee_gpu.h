@@ -62,6 +62,14 @@ extern "C" {
                                   * decoded bytes is passed through (mtz_stats.lz4_certified counts them);
                                   * the output bytes are the same either way */
 
+#define MTZ_FLAG_BLOCK_CKSUM 4u  /* VERIFY / COMPRESS / DECOMPRESS / RECOMPRESS (not PASSTHROUGH): check every
+                                  * DRR_WRITE against the on-disk block checksum `zfs send` copies into it
+                                  * (drr_key, fletcher4 keys only).  A block stored raw on disk must match
+                                  * its logical bytes: a mismatch fails the handle with MTZ_ECKSUM like a
+                                  * stream checksum.  A block stored LZ4 on disk is compared with the
+                                  * frame at hand: a mismatch is only counted (mtz_block_stats.frame_miss).
+                                  * Counters: mtz_get_block_stats */
+
 typedef struct mtz_handle mtz_handle;
 
 #define MTZ_MAX_DEVICES 16
@@ -107,6 +115,19 @@ typedef struct mtz_stats {
 	uint64_t lz4_certified; /* RECOMPRESS: records whose input frame was PROVEN to be the encoder's output
 	                           (kernels_lz4.cuh warp_lz4_certify) and passed through; the rest were re-encoded */
 } mtz_stats;
+
+/* MTZ_FLAG_BLOCK_CKSUM counters (all zero with the flag off).  A DRR_WRITE whose key the stage
+ * cannot check (not fletcher4, no key, encrypted, another on-disk compression, or no bytes at hand
+ * that the key covers) counts as skipped. */
+typedef struct mtz_block_stats {
+	uint32_t struct_size;       /* sizeof(mtz_block_stats), set by the caller */
+	uint32_t pad;
+	uint64_t logical_ok;        /* stored raw on disk: logical bytes match the key */
+	uint64_t frame_ok;          /* stored LZ4 on disk: the frame at hand matches the key */
+	uint64_t frame_miss;        /* ... does not: another encoder wrote the disk block */
+	uint64_t skipped;
+	uint64_t first_frame_miss;  /* stream index of the first frame miss, ~0 if none */
+} mtz_block_stats;
 
 /* One DRR record as seen by the kernels (32 B, little endian). */
 typedef struct mtz_rec {
@@ -182,6 +203,8 @@ int32_t mtz_cancel(mtz_handle *h);
  * (lib/backupServer.js:100-131 serialises the same object the sender mutates,
  * lib/backupSender.js:197-212): additive `job.gpu`, never read by the reference */
 int32_t mtz_get_stats(mtz_handle *h, mtz_stats *st);
+/* fills min(st->struct_size, sizeof(mtz_block_stats)) bytes */
+int32_t mtz_get_block_stats(mtz_handle *h, mtz_block_stats *st);
 /* running Fletcher-4 of the OUTPUT stream before DRR_END (== drr_end.drr_checksum) */
 int32_t mtz_end_checksum(mtz_handle *h, uint64_t out[4]);
 

@@ -52,8 +52,10 @@ function GpuFanoutStage(options) {
         ringBytes: options.ringBytes || 0,
         outRingBytes: options.outRingBytes || 0,
         batchBytes: options.batchBytes || 0,
-        slots: options.slots || 0
+        slots: options.slots || 0,
+        flags: options.blockChecksums ? 4 : 0     // gpu.blockChecksums: MTZ_FLAG_BLOCK_CKSUM
     });
+    this._blockChecksums = !!options.blockChecksums;
     this._peers = [];
     for (var i = 0; i < (options.peers || 1); i++) {
         this._addon.attach(this._h, i);
@@ -142,6 +144,9 @@ GpuFanoutStage.prototype._drain = function () {
         var fcb = this._finalCb;
         this._finalCb = null;
         this.stats = this._addon.stats(this._h);
+        if (this._blockChecksums) {
+            this.stats.blocks = this._addon.blockStats(this._h);
+        }
         this._cleanup();
         return (fcb());
     }

@@ -19,6 +19,7 @@ var stream = require('stream');
 var util = require('util');
 
 var MODES = { verify: 0, compress: 1, decompress: 2, recompress: 3, passthrough: 4 };
+var BLOCK_CKSUM = 4;        // MTZ_FLAG_BLOCK_CKSUM
 
 function GpuSnapshotStage(options) {
     if (!(this instanceof GpuSnapshotStage)) {
@@ -34,8 +35,10 @@ function GpuSnapshotStage(options) {
         ringBytes: options.ringBytes || 0,
         outRingBytes: options.outRingBytes || 0,
         batchBytes: options.batchBytes || 0,
-        slots: options.slots || 0
+        slots: options.slots || 0,
+        flags: options.blockChecksums ? BLOCK_CKSUM : 0   // gpu.blockChecksums
     });
+    this._blockChecksums = !!options.blockChecksums;
     this._pending = null;      // {chunk, off, cb} waiting for ring space
     this._flushCb = null;
     this._wantMore = true;     // cleared when push() returns false, set again by _read()
@@ -113,6 +116,9 @@ GpuSnapshotStage.prototype._drain = function () {
                 var fcb = this._flushCb;
                 this._flushCb = null;
                 this.stats = this._addon.stats(this._h);
+                if (this._blockChecksums) {
+                    this.stats.blocks = this._addon.blockStats(this._h);
+                }
                 this._cleanup();
                 if (fcb) { fcb(); }
                 return;

@@ -77,6 +77,7 @@ static napi_value Open(napi_env env, napi_callback_info info)
 	cfg.out_ring_bytes = get_u64_prop(env, argv[0], "outRingBytes");
 	cfg.batch_bytes = get_u64_prop(env, argv[0], "batchBytes");
 	cfg.n_slots = (uint32_t)get_u64_prop(env, argv[0], "slots");
+	cfg.flags = (uint32_t)get_u64_prop(env, argv[0], "flags");
 	const uint64_t mask = get_u64_prop(env, argv[0], "deviceMask");
 	for (int d = 0; d < MTZ_MAX_DEVICES; d++)
 		if (mask & (1ull << d)) cfg.devices[cfg.n_devices++] = d;
@@ -311,6 +312,31 @@ static napi_value Stats(napi_env env, napi_callback_info info)
 	return o;
 }
 
+// block-checksum counters (MTZ_FLAG_BLOCK_CKSUM): job.gpu.blocks.  A weak reference: the addon
+// still loads against a libmanatee_gpu.so older than the entry point (the ABI only grows), and
+// blockStats() returns undefined there.
+#pragma weak mtz_get_block_stats
+static napi_value BlockStats(napi_env env, napi_callback_info info)
+{
+	size_t argc = 1; napi_value argv[1];
+	NAPI_OK(napi_get_cb_info(env, info, &argc, argv, NULL, NULL));
+	mtz_handle *h = get_handle(env, argv[0]);
+	if (mtz_get_block_stats == NULL) return NULL;
+	mtz_block_stats st; memset(&st, 0, sizeof st);
+	st.struct_size = sizeof st;
+	int32_t rc = mtz_get_block_stats(h, &st);
+	if (rc != MTZ_OK) return throw_mtz(env, h, rc);
+	napi_value o, v; napi_create_object(env, &o);
+#define PUT(name, field) napi_create_double(env, (double)st.field, &v); napi_set_named_property(env, o, name, v)
+	PUT("logicalOk", logical_ok); PUT("frameOk", frame_ok); PUT("frameMiss", frame_miss);
+	PUT("skipped", skipped);
+#undef PUT
+	// ~0 (no miss) does not survive a double: -1 says "none"
+	napi_create_double(env, st.first_frame_miss == ~0ull ? -1.0 : (double)st.first_frame_miss, &v);
+	napi_set_named_property(env, o, "firstFrameMiss", v);
+	return o;
+}
+
 static napi_value EndChecksum(napi_env env, napi_callback_info info)
 {
 	size_t argc = 1; napi_value argv[1];
@@ -344,6 +370,7 @@ static napi_value Init(napi_env env, napi_value exports)
 		{"flush", 0, Flush, 0, 0, 0, napi_default, 0}, {"peek", 0, Peek, 0, 0, 0, napi_default, 0},
 		{"consume", 0, Consume, 0, 0, 0, napi_default, 0}, {"eventFd", 0, EventFd, 0, 0, 0, napi_default, 0},
 		{"stats", 0, Stats, 0, 0, 0, napi_default, 0}, {"close", 0, Close, 0, 0, 0, napi_default, 0},
+		{"blockStats", 0, BlockStats, 0, 0, 0, napi_default, 0},
 		{"endChecksum", 0, EndChecksum, 0, 0, 0, napi_default, 0},
 		{"watch", 0, Watch, 0, 0, 0, napi_default, 0}, {"unwatch", 0, Unwatch, 0, 0, 0, napi_default, 0},
 		{"attach", 0, Attach, 0, 0, 0, napi_default, 0}, {"cancel", 0, Cancel, 0, 0, 0, napi_default, 0},

@@ -17,6 +17,7 @@ MAX_DEVICES, MAX_PEERS = 16, 16
 MODE_VERIFY, MODE_COMPRESS, MODE_DECOMPRESS, MODE_RECOMPRESS, MODE_PASSTHROUGH = 0, 1, 2, 3, 4
 FLAG_DEFER_VERIFY = 1
 FLAG_REENCODE_ALL = 2
+FLAG_BLOCK_CKSUM = 4
 XCHG_FIRST, XCHG_LAST = 1, 2
 MODE_NAMES = {"verify": 0, "compress": 1, "decompress": 2, "recompress": 3, "passthrough": 4}
 
@@ -47,6 +48,15 @@ class Stats(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class BlockStats(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("pad", C.c_uint32), ("logical_ok", C.c_uint64),
+                ("frame_ok", C.c_uint64), ("frame_miss", C.c_uint64), ("skipped", C.c_uint64),
+                ("first_frame_miss", C.c_uint64)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_[2:]}
+
+
 class Rec(C.Structure):
     _fields_ = [("off", C.c_uint64), ("payload", C.c_uint32), ("type", C.c_uint32),
                 ("lsize", C.c_uint32), ("comp", C.c_uint32), ("resv", C.c_uint64)]
@@ -57,7 +67,7 @@ SYMBOLS = [
     "mtz_abi_version", "mtz_device_count", "mtz_open", "mtz_close", "mtz_last_error",
     "mtz_strerror", "mtz_ring_acquire", "mtz_ring_commit", "mtz_write", "mtz_flush",
     "mtz_out_peek", "mtz_out_consume", "mtz_read", "mtz_event_fd", "mtz_get_stats",
-    "mtz_end_checksum", "mtz_host_alloc", "mtz_host_free", "mtz_process_host",
+    "mtz_get_block_stats", "mtz_end_checksum", "mtz_host_alloc", "mtz_host_free", "mtz_process_host",
     "mtz_index_host", "mtz_dev_index", "mtz_dev_submit", "mtz_dev_aggregate",
     "mtz_dev_finish", "mtz_dev_reset", "mtz_dev_aggregate_async", "mtz_dev_finish_gathered", "mtz_set_carry",
     "mtz_k_lz4_decode", "mtz_k_lz4_encode",
@@ -109,6 +119,7 @@ def lib():
     L.mtz_read.argtypes = [H, vp, sz, C.POINTER(sz), i32]
     L.mtz_event_fd.argtypes = [H]
     L.mtz_get_stats.argtypes = [H, C.POINTER(Stats)]
+    L.mtz_get_block_stats.argtypes = [H, C.POINTER(BlockStats)]
     L.mtz_end_checksum.argtypes = [H, C.POINTER(u64 * 4)]
     L.mtz_host_alloc.argtypes = [sz, C.POINTER(vp)]
     L.mtz_host_free.argtypes = [vp]

@@ -1,0 +1,104 @@
+// kernels_block.cuh -- block-checksum check (MTZ_FLAG_BLOCK_CKSUM): every DRR_WRITE record
+// against the on-disk block checksum `zfs send` copies into its header ([EXTERNAL] dmu_send.c
+// dump_write(); SURVEY.md App. A.1):
+//   byte 48      drr_checksumtype (7 = fletcher4)
+//   bytes 56..87 drr_key.ddk_cksum, the block pointer's checksum of the PSIZE bytes on disk
+//   bytes 88..95 drr_key.ddk_prop: LSIZE bits 0..15 and PSIZE bits 16..31 as (size/512 - 1),
+//                on-disk compression bits 32..38, crypt bit 39
+// The stream's own Fletcher-4 chain is re-stamped by every re-encoding mode; this key is not, so it
+// ties the bytes a stage hands on to the bytes on the primary's disk.  The check reads only sums K1
+// already took (no pass over the stream bytes): the input's body sums start at byte 280, so the
+// eight checksum-field words in front of the payload are removed in closed form, and a payload
+// shorter than PSIZE is extended by zero words (shift_zeros).
+#pragma once
+#include "kernels_fletcher.cuh"
+
+namespace mtz {
+
+#define ZIO_CKSUM_FLETCHER4 7u
+#define BLK_DC_INHERIT 0u      // "stored raw": the key covers the logical block
+#define BLK_DC_OFF     2u
+#define BLK_DC_LZ4     15u     // the key covers ZFS's LZ4 frame, zero-padded to PSIZE
+
+struct BlockResult {           // device, mirrored to pinned host; zeroed per batch
+	unsigned long long logical_ok, frame_ok, frame_miss, skipped;
+	unsigned long long first_bad;    // stream index of the first logical mismatch, ~0 none
+	unsigned long long first_miss;   // stream index of the first frame mismatch, ~0 none
+};
+
+// zero-state sums of a segment's tail, given the sums of the whole segment and of its 8-word head
+// (the inverse of apply(head, tail) for a tail of n words)
+__host__ __device__ __forceinline__ Ck4 strip_head8(const Ck4 &whole, const Ck4 &head, uint64_t n)
+{
+	const uint64_t t2 = tri2(n), t3 = tri3(n);
+	Ck4 p;
+	p.a = whole.a - head.a;
+	p.b = whole.b - head.b - n * head.a;
+	p.c = whole.c - head.c - n * head.b - t2 * head.a;
+	p.d = whole.d - head.d - n * head.c - t2 * head.b - t3 * head.a;
+	return p;
+}
+
+// One thread per record.  `isums` are the input's K1 sums (body from byte 280), `orecs`/`osums`
+// the output records and their payload sums in the re-encoding modes (null in VERIFY).  Record r
+// is record `base + r` of the stream.
+#define BLK_THREADS 128
+__global__ void __launch_bounds__(BLK_THREADS)
+k_block_check(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs,
+    const RecSums *__restrict__ isums, const mtz_rec *__restrict__ orecs,
+    const RecSums *__restrict__ osums, uint32_t n, uint32_t mode, uint64_t base,
+    BlockResult *__restrict__ res)
+{
+	const uint32_t r = blockIdx.x * BLK_THREADS + threadIdx.x;
+	if (r >= n) return;
+	const mtz_rec rec = recs[r];
+	if (rec.type != DRR_WRITE_T) return;
+	const uint8_t *hdr = d_in + rec.off;
+	const uint64_t prop = *reinterpret_cast<const uint64_t *>(hdr + 88);
+	const uint64_t lsz = ((prop & 0xffffull) + 1ull) * 512ull;
+	const uint64_t psz = (((prop >> 16) & 0xffffull) + 1ull) * 512ull;
+	const uint32_t dc = (uint32_t)((prop >> 32) & 0x7full);
+	const bool raw_in = rec.comp == 0u, lz4_in = rec.comp == ZIO_LZ4;
+	const bool encodes = mode == MTZ_MODE_COMPRESS || mode == MTZ_MODE_RECOMPRESS;
+	// 0 skipped, 1 logical bytes, 2 disk frame;  src 0 input payload, 1 output payload
+	int what = 0, src = 0;
+	if (hdr[48] == ZIO_CKSUM_FLETCHER4 && prop != 0ull && !((prop >> 39) & 1ull) && lsz == rec.lsize) {
+		if ((dc == BLK_DC_INHERIT || dc == BLK_DC_OFF) && psz == lsz) {
+			if (raw_in) { what = 1; src = 0; }
+			else if (lz4_in && mode == MTZ_MODE_DECOMPRESS && osums != nullptr) { what = 1; src = 1; }
+		} else if (dc == BLK_DC_LZ4) {
+			if (lz4_in) { what = 2; src = 0; }
+			else if (raw_in && encodes && osums != nullptr) { what = 2; src = 1; }
+		}
+	}
+	if (what == 0) { atomicAdd(&res->skipped, 1ull); return; }
+	Ck4 sums;
+	uint64_t nbytes;
+	bool ok = true;
+	if (src == 0) {
+		const RecSums s = isums[r];
+		const Ck4 zero = { 0, 0, 0, 0 };
+		nbytes = (uint64_t)rec.payload;
+		sums = strip_head8(s.body, fold_cksum_words(zero, s.emb), s.nbody - 8u);
+	} else {
+		const mtz_rec o = orecs[r];
+		nbytes = (uint64_t)o.payload;
+		sums = osums[r].body;
+		// the stage's encoder stored the block raw where ZFS's stored a frame: not that encoder
+		if (what == 2 && o.comp != ZIO_LZ4) ok = false;
+	}
+	const uint64_t cover = (what == 1) ? lsz : psz;
+	if (nbytes > cover) ok = false;
+	if (ok) ok = ck_eq(shift_zeros(sums, (cover - nbytes) >> 2), load_ck(hdr + 56));
+	if (what == 1) {
+		if (ok) atomicAdd(&res->logical_ok, 1ull);
+		else atomicMin(&res->first_bad, (unsigned long long)(base + r));
+	} else if (ok) {
+		atomicAdd(&res->frame_ok, 1ull);
+	} else {
+		atomicAdd(&res->frame_miss, 1ull);
+		atomicMin(&res->first_miss, (unsigned long long)(base + r));
+	}
+}
+
+} // namespace mtz

@@ -14,8 +14,23 @@
 #include "kernels_lz4.cuh"
 #include "kernels_codec.cuh"
 #include "kernels_index.cuh"
+#include "kernels_block.cuh"
 
 namespace mtz {
+
+// block-check verdicts not yet folded into the handle: those of deferred batches wait for
+// mtz_dev_finish*, where the stream verdict of the same records surfaces
+struct BlockPending {
+	BlockResult r;
+	uint64_t obj = 0, off = 0;    // drr_object / drr_offset of record r.first_bad
+	BlockPending() { clear(); }
+	void clear()
+	{
+		r.logical_ok = r.frame_ok = r.frame_miss = r.skipped = 0;
+		r.first_bad = r.first_miss = ~0ull;
+		obj = off = 0;
+	}
+};
 
 // device scratch of one codec batch (modes COMPRESS / DECOMPRESS / RECOMPRESS)
 struct CodecBufs {
@@ -64,6 +79,7 @@ struct Slot {
 	Part *d_tiles = nullptr;      // scan spine scratch
 	ScanResult *d_res = nullptr;
 	ScanResult *h_res = nullptr;  // pinned
+	BlockResult *d_bres = nullptr, *h_bres = nullptr;   // MTZ_FLAG_BLOCK_CKSUM (h_: pinned)
 	cudaStream_t st = nullptr;
 	cudaStream_t st_k3 = nullptr;      // least-priority side stream of the LZ4 encoder (make_stream)
 	cudaEvent_t ev_start = nullptr, ev_done = nullptr;
@@ -142,6 +158,15 @@ struct mtz_handle {
 	mtz::StampStep *dv_all_steps = nullptr;
 	size_t dv_all_cap = 0;
 	uint8_t *dv_out = nullptr;
+
+	// MTZ_FLAG_BLOCK_CKSUM: results of the device API's submit, verdicts waiting for a finish,
+	// counters of the handle (under stats_mu)
+	mtz::BlockResult *dv_bres = nullptr, *dv_hbres = nullptr;
+	bool dv_bres_live = false;         // dv_bres holds the results of an unfinished mtz_dev_submit
+	const uint8_t *dv_in = nullptr;    // ... and the batch they refer to
+	const mtz_rec *dv_recs = nullptr;
+	mtz::BlockPending bpend;
+	mtz_block_stats bstats{};
 
 	mtz::IndexResult *d_ires = nullptr, *h_ires = nullptr;
 	mtz::IndexShared *d_ishared = nullptr;

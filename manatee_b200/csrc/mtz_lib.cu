@@ -7,6 +7,7 @@
 // (Fletcher-4 verify / LZ4 decode / LZ4 encode / re-stamp) -> pinned ring.
 // There is NO CPU fallback: without a usable device mtz_open fails MTZ_ENOGPU.
 #include <cstdarg>
+#include <cstddef>
 #include <cstdio>
 #include <cstring>
 #include <cstdlib>
@@ -205,6 +206,10 @@ static int32_t alloc_slot(mtz_handle *h, Slot &s, int di, size_t cap, size_t rec
 	MTZ_CU(h, cudaMalloc(&s.d_tiles, (rec_cap / SCAN_TILE + 2) * sizeof(Part)));
 	MTZ_CU(h, cudaMalloc(&s.d_res, sizeof(ScanResult)));
 	MTZ_CU(h, cudaHostAlloc(&s.h_res, sizeof(ScanResult), cudaHostAllocPortable));
+	if (h->cfg.flags & MTZ_FLAG_BLOCK_CKSUM) {
+		MTZ_CU(h, cudaMalloc(&s.d_bres, sizeof(BlockResult)));
+		MTZ_CU(h, cudaHostAlloc(&s.h_bres, sizeof(BlockResult), cudaHostAllocPortable));
+	}
 	MTZ_CU(h, make_stream(&s.st, true));
 	if (stream_priorities() && (h->cfg.mode == MTZ_MODE_COMPRESS || h->cfg.mode == MTZ_MODE_RECOMPRESS))
 		MTZ_CU(h, make_stream(&s.st_k3, false));
@@ -233,6 +238,8 @@ static void free_slot(Slot &s)
 	if (s.d_tiles) cudaFree(s.d_tiles);
 	if (s.d_res) cudaFree(s.d_res);
 	if (s.h_res) cudaFreeHost(s.h_res);
+	if (s.d_bres) cudaFree(s.d_bres);
+	if (s.h_bres) cudaFreeHost(s.h_bres);
 	if (s.st) cudaStreamDestroy(s.st);
 	if (s.st_k3) cudaStreamDestroy(s.st_k3);
 	if (s.ev_start) cudaEventDestroy(s.ev_start);
@@ -293,6 +300,8 @@ int32_t mtz_open(const mtz_config *cfg, mtz_handle **out)
 	if (full.n_devices > 1 && (full.flags & MTZ_FLAG_DEFER_VERIFY))
 		return fail(nullptr, MTZ_EINVAL, "a device group verifies in stream order; DEFER_VERIFY is the "
 		    "one-GPU-per-process shard form");
+	if ((full.flags & MTZ_FLAG_BLOCK_CKSUM) && full.mode == MTZ_MODE_PASSTHROUGH)
+		return fail(nullptr, MTZ_EINVAL, "PASSTHROUGH parses no record: BLOCK_CKSUM needs another mode");
 	const cudaDeviceProp &prop = props[0];
 
 	mtz_handle *h = new (std::nothrow) mtz_handle();
@@ -348,6 +357,11 @@ int32_t mtz_open(const mtz_config *cfg, mtz_handle **out)
 		MTZ_CU(h, cudaHostAlloc(&h->dv_hres, sizeof(ScanResult), cudaHostAllocPortable));
 		MTZ_CU(h, cudaEventCreate(&h->dv_k1a));
 		MTZ_CU(h, cudaEventCreate(&h->dv_k1b));
+		if (full.flags & MTZ_FLAG_BLOCK_CKSUM) {
+			MTZ_CU(h, cudaMalloc(&h->dv_bres, sizeof(BlockResult)));
+			MTZ_CU(h, cudaHostAlloc(&h->dv_hbres, sizeof(BlockResult), cudaHostAllocPortable));
+			h->bstats.first_frame_miss = ~0ull;
+		}
 		return MTZ_OK;
 	};
 	rc = init();
@@ -401,6 +415,8 @@ int32_t mtz_close(mtz_handle *h)
 	if (h->h_ires) cudaFreeHost(h->h_ires);
 	if (h->dv_k1a) cudaEventDestroy(h->dv_k1a);
 	if (h->dv_k1b) cudaEventDestroy(h->dv_k1b);
+	if (h->dv_bres) cudaFree(h->dv_bres);
+	if (h->dv_hbres) cudaFreeHost(h->dv_hbres);
 	for (auto &s : h->slots) { cudaSetDevice(h->devs[s.di].device); free_slot(s); }
 	cudaSetDevice(h->device);
 	if (h->dv_sums) cudaFree(h->dv_sums);
@@ -423,6 +439,21 @@ int32_t mtz_get_stats(mtz_handle *h, mtz_stats *st)
 	if (h == nullptr || st == nullptr) return MTZ_EINVAL;
 	std::lock_guard<std::mutex> g(h->stats_mu);
 	*st = h->stats;
+	return MTZ_OK;
+}
+
+int32_t mtz_get_block_stats(mtz_handle *h, mtz_block_stats *st)
+{
+	if (h == nullptr || st == nullptr || st->struct_size < 2 * sizeof(uint32_t)) return MTZ_EINVAL;
+	mtz_block_stats b;
+	memset(&b, 0, sizeof b);
+	if (h->cfg.flags & MTZ_FLAG_BLOCK_CKSUM) {
+		std::lock_guard<std::mutex> g(h->stats_mu);
+		b = h->bstats;
+	}
+	const size_t n = std::min((size_t)st->struct_size, sizeof b);
+	b.struct_size = (uint32_t)n;
+	memcpy(st, &b, n);
 	return MTZ_OK;
 }
 
@@ -511,6 +542,71 @@ static int32_t launch_scan(mtz_handle *h, cudaStream_t st, const RecSums *d_sums
 	MTZ_CU(h, cudaGetLastError());
 	count_launch(h, phase == 1 ? 3 : 2);
 	return MTZ_OK;
+}
+
+// ------------------------------------------------- block checksums (drr_key) --
+static bool block_on(const mtz_handle *h) { return (h->cfg.flags & MTZ_FLAG_BLOCK_CKSUM) != 0; }
+
+static int32_t block_reset(mtz_handle *h, cudaStream_t st, BlockResult *bres)
+{
+	MTZ_CU(h, cudaMemsetAsync(bres, 0, offsetof(BlockResult, first_bad), st));
+	MTZ_CU(h, cudaMemsetAsync(&bres->first_bad, 0xff, 2 * sizeof(unsigned long long), st));
+	return MTZ_OK;
+}
+
+// k_block_check over records [0, nrec) of a (sub-)batch, record 0 being stream record `base`.  Not
+// counted in mtz_stats.kernel_launches: the flag leaves every mtz_stats field as it is.
+static int32_t launch_block(mtz_handle *h, cudaStream_t st, const uint8_t *d_in, const mtz_rec *d_recs,
+    const RecSums *isums, const mtz_rec *orecs, const RecSums *osums, size_t nrec, uint64_t base,
+    BlockResult *bres)
+{
+	if (nrec == 0) return MTZ_OK;
+	const unsigned grid = (unsigned)((nrec + BLK_THREADS - 1) / BLK_THREADS);
+	k_block_check<<<grid, BLK_THREADS, 0, st>>>(d_in, d_recs, isums, orecs, osums, (uint32_t)nrec,
+	    h->cfg.mode, base, bres);
+	MTZ_CU(h, cudaGetLastError());
+	return MTZ_OK;
+}
+
+// Merge a batch's results (host copy) into `p`; on a mismatch read drr_object / drr_offset of the
+// failing record from the device copy of its header (`off` = header offset in d_in).  Synchronous,
+// only on the failure path.
+static int32_t block_take(mtz_handle *h, BlockPending &p, const BlockResult &r, const uint8_t *d_in,
+    uint64_t off)
+{
+	p.r.logical_ok += r.logical_ok; p.r.frame_ok += r.frame_ok;
+	p.r.frame_miss += r.frame_miss; p.r.skipped += r.skipped;
+	p.r.first_miss = std::min(p.r.first_miss, r.first_miss);
+	if (r.first_bad < p.r.first_bad) {
+		uint64_t w[4];
+		MTZ_CU(h, cudaMemcpy(w, d_in + off + 8, sizeof w, cudaMemcpyDeviceToHost));
+		p.r.first_bad = r.first_bad;
+		p.obj = w[0]; p.off = w[2];
+	}
+	return MTZ_OK;
+}
+
+// Fold the pending block verdicts into the handle.  `stream_bad` = first record of the same
+// records whose stream checksum failed (~0 none): the first failing record in stream order is the
+// one reported, and a record that fails both reports its stream checksum.
+static int32_t block_fold(mtz_handle *h, BlockPending &p, uint64_t stream_bad)
+{
+	const BlockPending q = p;
+	p.clear();
+	{
+		std::lock_guard<std::mutex> g(h->stats_mu);
+		h->bstats.logical_ok += q.r.logical_ok; h->bstats.frame_ok += q.r.frame_ok;
+		h->bstats.frame_miss += q.r.frame_miss; h->bstats.skipped += q.r.skipped;
+		h->bstats.first_frame_miss = std::min<uint64_t>(h->bstats.first_frame_miss, q.r.first_miss);
+	}
+	if (q.r.first_bad == ~0ull || q.r.first_bad >= stream_bad) return MTZ_OK;
+	{
+		std::lock_guard<std::mutex> g(h->stats_mu);
+		if (q.r.first_bad < h->stats.bad_record) h->stats.bad_record = q.r.first_bad;
+	}
+	return fail(h, MTZ_ECKSUM, "block checksum mismatch at record %llu (object %llu, offset %llu): "
+	    "the bytes differ from the block on disk", (unsigned long long)q.r.first_bad,
+	    (unsigned long long)q.obj, (unsigned long long)q.off);
 }
 
 static int32_t ensure_dv_sums(mtz_handle *h, size_t need, cudaStream_t st)
@@ -672,9 +768,12 @@ static int32_t codec_launch_enc(mtz_handle *h, cudaStream_t st, CodecBufs &cb, s
 // Part 2: layout, assemble into d_out + *cb.d_outpos (the running output offset
 // lives on the device so sub-batches chain without a host round trip), sums of
 // the output records, and the sequential stamp chain from h->d_carry_out.
+// With `bres` the block check runs on the output sums as well (`isums` = the input's sums of these
+// records, `bbase` = stream index of the first of them).
 static int32_t codec_launch_post(mtz_handle *h, cudaStream_t st, CodecBufs &cb, const uint8_t *d_in,
     const mtz_rec *d_recs, size_t nrec, uint8_t *d_out, uint32_t rec_base,
-    mtz_rec *all_orecs = nullptr, RecSums *all_osums = nullptr, Ck4 *d_carry_out = nullptr)
+    mtz_rec *all_orecs = nullptr, RecSums *all_osums = nullptr, Ck4 *d_carry_out = nullptr,
+    const RecSums *isums = nullptr, uint64_t bbase = 0, BlockResult *bres = nullptr)
 {
 	if (nrec == 0) return MTZ_OK;
 	if (d_carry_out == nullptr) d_carry_out = h->d_carry_out;
@@ -692,6 +791,10 @@ static int32_t codec_launch_post(mtz_handle *h, cudaStream_t st, CodecBufs &cb, 
 	MTZ_CU(h, cudaGetLastError());
 	// output records of a codec batch are smaller than the logical size: decide by the input's
 	launch_k1_kernel(h, st, d_out, orecs, n, osums, 312u, cb.avg_out_rec);
+	if (bres != nullptr) {
+		const int32_t rc = launch_block(h, st, d_in, d_recs, isums, orecs, osums, nrec, bbase, bres);
+		if (rc != MTZ_OK) return rc;
+	}
 	if (all_osums == nullptr) {
 		const unsigned gp = (n + 127u) / 128u;
 		k_stamp_prep<<<gp, 128, 0, st>>>(orecs, osums, n, cb.steps);
@@ -714,9 +817,13 @@ int32_t mtz_dev_reset(mtz_handle *h)
 	MTZ_CU(h, cudaStreamSynchronize(h->st));
 	h->records_done = 0;
 	h->dv_nrec = 0; h->dv_in_bytes = 0;
+	h->dv_bres_live = false;
+	h->bpend.clear();
 	std::lock_guard<std::mutex> g(h->stats_mu);
 	h->stats = mtz_stats();
 	h->stats.bad_record = ~0ull;
+	h->bstats = mtz_block_stats();
+	if (block_on(h)) h->bstats.first_frame_miss = ~0ull;
 	return MTZ_OK;
 }
 
@@ -747,7 +854,17 @@ int32_t mtz_dev_submit(mtz_handle *h, const void *d_in, size_t in_bytes,
 	rc = launch_k1(h, st, (const uint8_t *)d_in, d_recs, nrec, h->dv_sums, h->dv_k1a, h->dv_k1b,
 	    nrec ? in_bytes / nrec : 0);
 	h->dv_timed = (rc == MTZ_OK && nrec > 0);
-	if (rc != MTZ_OK || !is_codec_mode(h->cfg.mode)) return rc;
+	if (rc != MTZ_OK) return rc;
+	h->dv_bres_live = block_on(h) && nrec > 0;
+	if (h->dv_bres_live) {
+		h->dv_in = (const uint8_t *)d_in; h->dv_recs = d_recs;
+		rc = block_reset(h, st, h->dv_bres);
+		if (rc == MTZ_OK && !is_codec_mode(h->cfg.mode))
+			rc = launch_block(h, st, (const uint8_t *)d_in, d_recs, h->dv_sums, nullptr, nullptr, nrec,
+			    h->dv_first, h->dv_bres);
+		if (rc != MTZ_OK) return rc;
+	}
+	if (!is_codec_mode(h->cfg.mode)) return MTZ_OK;
 
 	// ---- re-encoding modes: bounded-scratch sub-batches, output chained on device.
 	// Two scratch sets and a second stream: plan+K2+K3 of sub-batch k+1 (stream st)
@@ -841,7 +958,8 @@ int32_t mtz_dev_submit(mtz_handle *h, const void *d_in, size_t in_bytes,
 		MTZ_CU(h, cudaStreamWaitEvent(h->st_post, h->ev_pre[b], 0));
 		rc = codec_launch_post(h, h->st_post, cb, (const uint8_t *)d_in, d_recs + i0, i1 - i0,
 		    (uint8_t *)d_out, (uint32_t)i0, defer ? h->dv_all_orecs : nullptr,
-		    defer ? h->dv_all_osums : nullptr);
+		    defer ? h->dv_all_osums : nullptr, nullptr, h->dv_sums + i0, h->dv_first + i0,
+		    h->dv_bres_live ? h->dv_bres : nullptr);
 		if (rc != MTZ_OK) return rc;
 		MTZ_CU(h, cudaEventRecord(h->ev_post[b], h->st_post));
 		used[b] = true;
@@ -869,8 +987,9 @@ int32_t mtz_dev_aggregate(mtz_handle *h, uint64_t agg[5])
 	return MTZ_OK;
 }
 
+// `bp`: block-check verdicts of the same records (MTZ_FLAG_BLOCK_CKSUM), folded in with them
 static int32_t account_result(mtz_handle *h, const ScanResult &r, uint64_t first_rec, size_t nrec,
-    size_t bytes_in, size_t bytes_out)
+    size_t bytes_in, size_t bytes_out, BlockPending *bp = nullptr)
 {
 	{
 		std::lock_guard<std::mutex> g(h->stats_mu);
@@ -882,6 +1001,10 @@ static int32_t account_result(mtz_handle *h, const ScanResult &r, uint64_t first
 			h->stats.end_seen = 1;
 			memcpy(h->end_ck, &r.end_ck, 32);
 		}
+	}
+	if (bp != nullptr) {
+		const int32_t rc = block_fold(h, *bp, r.bad != 0xffffffffu ? first_rec + r.bad : ~0ull);
+		if (rc != MTZ_OK) return rc;
 	}
 	if (r.bad != 0xffffffffu) {
 		const uint64_t bad = first_rec + r.bad;
@@ -1057,7 +1180,20 @@ static int32_t dev_finish_impl(mtz_handle *h, const uint64_t carry_in[4], const 
 		MTZ_CU(h, cudaMemcpyAsync(h->dv_cb.h_cres, h->dv_cb.d_cres, sizeof(CodecResult), cudaMemcpyDeviceToHost, st));
 		MTZ_CU(h, cudaMemcpyAsync(h->dv_cb.h_ores, h->dv_cb.d_ores, sizeof(ScanResult), cudaMemcpyDeviceToHost, st));
 	}
+	if (h->dv_bres_live)
+		MTZ_CU(h, cudaMemcpyAsync(h->dv_hbres, h->dv_bres, sizeof(BlockResult), cudaMemcpyDeviceToHost, st));
 	MTZ_CU(h, cudaStreamSynchronize(st));
+	if (h->dv_bres_live) {
+		// the block verdicts of mtz_dev_submit's records (deferred ring batches were merged at harvest)
+		h->dv_bres_live = false;
+		const BlockResult br = *h->dv_hbres;
+		mtz_rec fr;
+		fr.off = 0;
+		if (br.first_bad != ~0ull)
+			MTZ_CU(h, cudaMemcpy(&fr, h->dv_recs + (br.first_bad - h->dv_first), sizeof fr, cudaMemcpyDeviceToHost));
+		rc = block_take(h, h->bpend, br, h->dv_in, fr.off);
+		if (rc != MTZ_OK) return rc;
+	}
 	if (codec && h->dv_nrec > 0) {
 		float cm = 0;
 		if (cudaEventElapsedTime(&cm, h->dv_c0, h->dv_c1) == cudaSuccess) {
@@ -1104,7 +1240,7 @@ static int32_t dev_finish_impl(mtz_handle *h, const uint64_t carry_in[4], const 
 		h->stats.lz4_certified += c.n_cert;
 	}
 	if (out_bytes) *out_bytes = ob;
-	rc = account_result(h, r, h->dv_first, h->dv_nrec, h->dv_in_bytes, ob);
+	rc = account_result(h, r, h->dv_first, h->dv_nrec, h->dv_in_bytes, ob, block_on(h) ? &h->bpend : nullptr);
 	if (rc == MTZ_OK) h->records_done = h->dv_first + h->dv_nrec;
 	if (rc == MTZ_OK && codec && h->dv_nrec > 0 && h->dv_cb.h_ores->end_seen) {
 		std::lock_guard<std::mutex> g(h->stats_mu);
@@ -1233,6 +1369,14 @@ static int32_t harvest(mtz_handle *h, Slot &s)
 		if (cok) h->stats.codec_ms += cm;
 		if (k3ok) { h->stats.k3_ms += k3; h->stats.k3_launches += 1; }
 	}
+	BlockPending bp;
+	if (block_on(h) && s.nrec > 0) {
+		const BlockResult &br = *s.h_bres;
+		const uint64_t off = br.first_bad != ~0ull ? s.h_recs[br.first_bad - s.first_rec].off : 0;
+		// deferred batches: the verdict waits for mtz_dev_finish, with the stream verdict
+		int32_t rc = block_take(h, (h->cfg.flags & MTZ_FLAG_DEFER_VERIFY) ? h->bpend : bp, br, s.d_in, off);
+		if (rc != MTZ_OK) return rc;
+	}
 	if (h->cfg.mode == MTZ_MODE_PASSTHROUGH || (h->cfg.flags & MTZ_FLAG_DEFER_VERIFY)) {
 		std::lock_guard<std::mutex> g(h->stats_mu);
 		h->stats.batches += 1; h->stats.bytes_in += s.bytes; h->stats.bytes_out += s.out_bytes;
@@ -1256,7 +1400,8 @@ static int32_t harvest(mtz_handle *h, Slot &s)
 		h->stats.lz4_encoded += c.n_enc;
 		h->stats.lz4_certified += c.n_cert;
 	}
-	int32_t rc = account_result(h, *s.h_res, s.first_rec, s.nrec, s.bytes, s.out_bytes);
+	int32_t rc = account_result(h, *s.h_res, s.first_rec, s.nrec, s.bytes, s.out_bytes,
+	    block_on(h) ? &bp : nullptr);
 	if (rc == MTZ_OK && codec && s.nrec > 0 && s.cb.h_ores->end_seen) {
 		std::lock_guard<std::mutex> g(h->stats_mu);
 		h->stats.end_seen = 1;
@@ -1290,6 +1435,14 @@ static int32_t submit_batch(mtz_handle *h, Slot &s, const uint8_t *p0, size_t n0
 		rc = launch_k1(h, s.st, s.d_in, s.d_recs, nrec, h->dv_sums + h->dv_nrec, s.ev_k1a, s.ev_k1b,
 		    nrec ? bytes / nrec : 0);
 		if (rc != MTZ_OK) return rc;
+		// the block check needs no running checksum: it runs now, its verdict waits with the stream's
+		if (block_on(h) && nrec > 0) {
+			rc = block_reset(h, s.st, s.d_bres);
+			if (rc == MTZ_OK)
+				rc = launch_block(h, s.st, s.d_in, s.d_recs, h->dv_sums + h->dv_nrec, nullptr, nullptr, nrec,
+				    s.first_rec, s.d_bres);
+			if (rc != MTZ_OK) return rc;
+		}
 		if (h->dv_nrec == 0) h->dv_first = s.first_rec;
 		h->dv_nrec += nrec; h->dv_in_bytes += bytes; h->dv_st = h->st;
 	} else if (h->cfg.mode != MTZ_MODE_PASSTHROUGH) {
@@ -1297,6 +1450,13 @@ static int32_t submit_batch(mtz_handle *h, Slot &s, const uint8_t *p0, size_t n0
 		rc = launch_k1(h, s.st, s.d_in, s.d_recs, nrec, s.d_sums, s.ev_k1a, s.ev_k1b,
 		    nrec ? bytes / nrec : 0);
 		if (rc != MTZ_OK) return rc;
+		if (block_on(h) && nrec > 0) {
+			// VERIFY checks the input here; the codec modes after the output's sums (codec_launch_post)
+			rc = block_reset(h, s.st, s.d_bres);
+			if (rc == MTZ_OK && !is_codec_mode(h->cfg.mode))
+				rc = launch_block(h, s.st, s.d_in, s.d_recs, s.d_sums, nullptr, nullptr, nrec, s.first_rec, s.d_bres);
+			if (rc != MTZ_OK) return rc;
+		}
 		if (is_codec_mode(h->cfg.mode)) {
 			rc = codec_reset(h, s.st, s.cb);
 			if (rc != MTZ_OK) return rc;
@@ -1323,7 +1483,7 @@ static int32_t submit_batch(mtz_handle *h, Slot &s, const uint8_t *p0, size_t n0
 		MTZ_CU(h, cudaMemcpyAsync(dc.d_carry_in, &s.d_res->carry, 32, cudaMemcpyDeviceToDevice, s.st));
 		if (is_codec_mode(h->cfg.mode)) {
 			rc = codec_launch_post(h, s.st, s.cb, s.d_in, s.d_recs, nrec, s.d_out, 0u, nullptr, nullptr,
-			    dc.d_carry_out);
+			    dc.d_carry_out, s.d_sums, s.first_rec, (block_on(h) && nrec > 0) ? s.d_bres : nullptr);
 			if (rc != MTZ_OK) return rc;
 			MTZ_CU(h, cudaMemcpyAsync(s.cb.h_cres, s.cb.d_cres, sizeof(CodecResult), cudaMemcpyDeviceToHost, s.st));
 			MTZ_CU(h, cudaMemcpyAsync(s.cb.h_ores, s.cb.d_ores, sizeof(ScanResult), cudaMemcpyDeviceToHost, s.st));
@@ -1332,6 +1492,8 @@ static int32_t submit_batch(mtz_handle *h, Slot &s, const uint8_t *p0, size_t n0
 		h->prev_scan_slot = (int)(&s - h->slots.data());
 		MTZ_CU(h, cudaMemcpyAsync(s.h_res, s.d_res, sizeof(ScanResult), cudaMemcpyDeviceToHost, s.st));
 	}
+	if (block_on(h) && nrec > 0)
+		MTZ_CU(h, cudaMemcpyAsync(s.h_bres, s.d_bres, sizeof(BlockResult), cudaMemcpyDeviceToHost, s.st));
 	if (host_out != nullptr && !is_codec_mode(h->cfg.mode))
 		MTZ_CU(h, cudaMemcpyAsync(host_out, s.d_in, bytes, cudaMemcpyDeviceToHost, s.st));
 	MTZ_CU(h, cudaEventRecord(s.ev_done, s.st));

@@ -130,7 +130,16 @@ class BackupSender(object):
             g["mode"] = "verify"
         return GpuSnapshotStage(g["mode"], device=g.get("device", 0), devices=g.get("devices"),
                                 ring_bytes=g.get("ringBytes", 0), batch_bytes=g.get("batchBytes", 0),
-                                out_ring_bytes=g.get("outRingBytes", 0), n_slots=g.get("slots", 0))
+                                out_ring_bytes=g.get("outRingBytes", 0), n_slots=g.get("slots", 0),
+                                block_checksums=bool(g.get("blockChecksums")))
+
+    def _stage_stats(self, stage):
+        """job.gpu: the stage counters, plus `blocks` (block-checksum counters) with
+        gpu.blockChecksums set"""
+        st = stage.stats()
+        if self._gpu.get("blockChecksums"):
+            st["blocks"] = stage.block_stats()
+        return st
 
     def _send_group(self, jobs):
         """One zfs send + one stage pass teed to every job's socket (coalesced restore)."""
@@ -279,7 +288,7 @@ class BackupSender(object):
                     zfsSend.terminate()
                 for t_ in tds:
                     t_.join()
-                backupJob["gpu"] = stage.stats()
+                backupJob["gpu"] = self._stage_stats(stage)
                 if len(dead) == len(peer_socks) and not pump_err:
                     pump_err.append(OSError("every coalesced receiver went away"))
             elif stage is None:
@@ -319,7 +328,7 @@ class BackupSender(object):
                     # error (lib/backupSender.js:230-233) BEFORE waiting for it.
                     zfsSend.terminate()
                 td.join()
-                backupJob["gpu"] = stage.stats()              # additive field (SURVEY 8f f4)
+                backupJob["gpu"] = self._stage_stats(stage)   # additive field (SURVEY 8f f4)
             code = zfsSend.wait()
             te.join(2)
             if pump_err:

@@ -119,7 +119,8 @@ class ZfsClient(object):
         g = self._gpu
         return GpuSnapshotStage(mode or g["mode"], device=g.get("device", 0),
                                 ring_bytes=g.get("ringBytes", 0), batch_bytes=g.get("batchBytes", 0),
-                                out_ring_bytes=g.get("outRingBytes", 0), n_slots=g.get("slots", 0))
+                                out_ring_bytes=g.get("outRingBytes", 0), n_slots=g.get("slots", 0),
+                                block_checksums=bool(g.get("blockChecksums")))
 
     def _wire_mode(self, serverUrl, jobPath):
         """Which stage to put in the pipe for THIS job (SURVEY.md 8f f2).  A receiver configured
@@ -233,6 +234,8 @@ class ZfsClient(object):
                     abort.set()
                 if stage is not None:
                     self._gpuStats = stage.stats()
+                    if self._gpu.get("blockChecksums"):
+                        self._gpuStats["blocks"] = stage.block_stats()
                     stage.close()
                 if conn is not None:
                     conn.close()

@@ -20,9 +20,13 @@ class GpuSnapshotStage(object):
     """One stage instance == one mtz_handle == one stream (like one Transform)."""
 
     def __init__(self, mode="verify", device=0, ring_bytes=0, batch_bytes=0, n_slots=0,
-                 out_ring_bytes=0, flags=0, devices=None):
+                 out_ring_bytes=0, flags=0, devices=None, block_checksums=False):
         """``devices`` = CUDA ordinals of a device group: the GPUs of one box run as ONE stage,
-        batch b of the stream on ``devices[b % len(devices)]`` (mtz_config.devices[])."""
+        batch b of the stream on ``devices[b % len(devices)]`` (mtz_config.devices[]).
+        ``block_checksums`` = MTZ_FLAG_BLOCK_CKSUM: every DRR_WRITE is also checked against the
+        on-disk block checksum the stream carries (``block_stats()``)."""
+        if block_checksums:
+            flags |= N.FLAG_BLOCK_CKSUM
         self._L = N.lib()
         self._h = C.c_void_p()
         cfg = N.Config()
@@ -74,6 +78,14 @@ class GpuSnapshotStage(object):
     def stats(self):
         st = N.Stats()
         self._check(self._L.mtz_get_stats(self._h, C.byref(st)))
+        return st.as_dict()
+
+    def block_stats(self):
+        """Block-checksum counters (mtz_get_block_stats); all zero without ``block_checksums``.
+        ``first_frame_miss`` is the stream index of the first frame miss, 2**64-1 if none."""
+        st = N.BlockStats()
+        st.struct_size = C.sizeof(N.BlockStats)
+        self._check(self._L.mtz_get_block_stats(self._h, C.byref(st)))
         return st.as_dict()
 
     def end_checksum(self):
