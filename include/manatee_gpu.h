@@ -70,6 +70,11 @@ extern "C" {
                                   * frame at hand: a mismatch is only counted (mtz_block_stats.frame_miss).
                                   * Counters: mtz_get_block_stats */
 
+#define MTZ_FLAG_BLOCK_SHA256 8u /* with MTZ_FLAG_BLOCK_CKSUM only (MTZ_EINVAL without it): also check the
+                                  * records whose key is a SHA-256 (drr_checksumtype 8, checksum=sha256),
+                                  * by the same rules and with the same consequences as fletcher4 keys;
+                                  * mtz_block_stats.sha256 counts them.  Without this flag they are skipped */
+
 typedef struct mtz_handle mtz_handle;
 
 #define MTZ_MAX_DEVICES 16
@@ -117,8 +122,8 @@ typedef struct mtz_stats {
 } mtz_stats;
 
 /* MTZ_FLAG_BLOCK_CKSUM counters (all zero with the flag off).  A DRR_WRITE whose key the stage
- * cannot check (not fletcher4, no key, encrypted, another on-disk compression, or no bytes at hand
- * that the key covers) counts as skipped. */
+ * cannot check (not fletcher4 -- or sha256 with MTZ_FLAG_BLOCK_SHA256 --, no key, encrypted, another
+ * on-disk compression, or no bytes at hand that the key covers) counts as skipped. */
 typedef struct mtz_block_stats {
 	uint32_t struct_size;       /* sizeof(mtz_block_stats), set by the caller */
 	uint32_t pad;
@@ -127,6 +132,8 @@ typedef struct mtz_block_stats {
 	uint64_t frame_miss;        /* ... does not: another encoder wrote the disk block */
 	uint64_t skipped;
 	uint64_t first_frame_miss;  /* stream index of the first frame miss, ~0 if none */
+	uint64_t sha256;            /* MTZ_FLAG_BLOCK_SHA256: records compared by SHA-256 (also counted above,
+	                               or the cause of the failure) */
 } mtz_block_stats;
 
 /* One DRR record as seen by the kernels (32 B, little endian). */

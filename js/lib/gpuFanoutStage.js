@@ -53,7 +53,8 @@ function GpuFanoutStage(options) {
         outRingBytes: options.outRingBytes || 0,
         batchBytes: options.batchBytes || 0,
         slots: options.slots || 0,
-        flags: options.blockChecksums ? 4 : 0     // gpu.blockChecksums: MTZ_FLAG_BLOCK_CKSUM
+        flags: (options.blockChecksums ? 4 : 0) |   // gpu.blockChecksums: MTZ_FLAG_BLOCK_CKSUM
+            (options.blockSha256 ? 8 : 0)          // gpu.blockSha256: MTZ_FLAG_BLOCK_SHA256
     });
     this._blockChecksums = !!options.blockChecksums;
     this._peers = [];

@@ -20,6 +20,7 @@ var util = require('util');
 
 var MODES = { verify: 0, compress: 1, decompress: 2, recompress: 3, passthrough: 4 };
 var BLOCK_CKSUM = 4;        // MTZ_FLAG_BLOCK_CKSUM
+var BLOCK_SHA256 = 8;       // MTZ_FLAG_BLOCK_SHA256 (with BLOCK_CKSUM only)
 
 function GpuSnapshotStage(options) {
     if (!(this instanceof GpuSnapshotStage)) {
@@ -36,7 +37,8 @@ function GpuSnapshotStage(options) {
         outRingBytes: options.outRingBytes || 0,
         batchBytes: options.batchBytes || 0,
         slots: options.slots || 0,
-        flags: options.blockChecksums ? BLOCK_CKSUM : 0   // gpu.blockChecksums
+        flags: (options.blockChecksums ? BLOCK_CKSUM : 0) |   // gpu.blockChecksums
+            (options.blockSha256 ? BLOCK_SHA256 : 0)         // gpu.blockSha256
     });
     this._blockChecksums = !!options.blockChecksums;
     this._pending = null;      // {chunk, off, cb} waiting for ring space

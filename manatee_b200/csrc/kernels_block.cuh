@@ -1,7 +1,7 @@
 // kernels_block.cuh -- block-checksum check (MTZ_FLAG_BLOCK_CKSUM): every DRR_WRITE record
 // against the on-disk block checksum `zfs send` copies into its header ([EXTERNAL] dmu_send.c
 // dump_write(); SURVEY.md App. A.1):
-//   byte 48      drr_checksumtype (7 = fletcher4)
+//   byte 48      drr_checksumtype (7 = fletcher4, 8 = sha256: kernels_sha256.cuh)
 //   bytes 56..87 drr_key.ddk_cksum, the block pointer's checksum of the PSIZE bytes on disk
 //   bytes 88..95 drr_key.ddk_prop: LSIZE bits 0..15 and PSIZE bits 16..31 as (size/512 - 1),
 //                on-disk compression bits 32..38, crypt bit 39
@@ -16,12 +16,14 @@
 namespace mtz {
 
 #define ZIO_CKSUM_FLETCHER4 7u
+#define ZIO_CKSUM_SHA256    8u
 #define BLK_DC_INHERIT 0u      // "stored raw": the key covers the logical block
 #define BLK_DC_OFF     2u
 #define BLK_DC_LZ4     15u     // the key covers ZFS's LZ4 frame, zero-padded to PSIZE
 
 struct BlockResult {           // device, mirrored to pinned host; zeroed per batch
 	unsigned long long logical_ok, frame_ok, frame_miss, skipped;
+	unsigned long long sha256;       // records compared by k_block_sha256 (kernels_sha256.cuh)
 	unsigned long long first_bad;    // stream index of the first logical mismatch, ~0 none
 	unsigned long long first_miss;   // stream index of the first frame mismatch, ~0 none
 };
@@ -39,39 +41,75 @@ __host__ __device__ __forceinline__ Ck4 strip_head8(const Ck4 &whole, const Ck4 
 	return p;
 }
 
+// What a record's key lets the stage compare, decided from its header alone, for keys of type
+// `ctype`: `what` 0 skipped, 1 the logical block, 2 the disk frame; `src` 0 the input payload, 1 the
+// output payload.  `have_out` = the output records of a re-encoding mode are at hand.  Every key
+// type that is checked goes through this one table.
+struct BlockClass {
+	int what, src;
+	uint64_t lsz, psz;
+};
+
+__device__ __forceinline__ BlockClass block_classify(const uint8_t *hdr, const mtz_rec &rec, uint32_t mode,
+    bool have_out, uint32_t ctype)
+{
+	const uint64_t prop = *reinterpret_cast<const uint64_t *>(hdr + 88);
+	BlockClass c;
+	c.lsz = ((prop & 0xffffull) + 1ull) * 512ull;
+	c.psz = (((prop >> 16) & 0xffffull) + 1ull) * 512ull;
+	c.what = 0; c.src = 0;
+	const uint32_t dc = (uint32_t)((prop >> 32) & 0x7full);
+	const bool raw_in = rec.comp == 0u, lz4_in = rec.comp == ZIO_LZ4;
+	const bool encodes = mode == MTZ_MODE_COMPRESS || mode == MTZ_MODE_RECOMPRESS;
+	if (hdr[48] == ctype && prop != 0ull && !((prop >> 39) & 1ull) && c.lsz == rec.lsize) {
+		if ((dc == BLK_DC_INHERIT || dc == BLK_DC_OFF) && c.psz == c.lsz) {
+			if (raw_in) { c.what = 1; c.src = 0; }
+			else if (lz4_in && mode == MTZ_MODE_DECOMPRESS && have_out) { c.what = 1; c.src = 1; }
+		} else if (dc == BLK_DC_LZ4) {
+			if (lz4_in) { c.what = 2; c.src = 0; }
+			else if (raw_in && encodes && have_out) { c.what = 2; c.src = 1; }
+		}
+	}
+	return c;
+}
+
+// The verdict of a compared record, `ok` = the bytes match the key.  Record `idx` of the stream.
+__device__ __forceinline__ void block_verdict(BlockResult *res, int what, bool ok, uint64_t idx)
+{
+	if (what == 1) {
+		if (ok) atomicAdd(&res->logical_ok, 1ull);
+		else atomicMin(&res->first_bad, (unsigned long long)idx);
+	} else if (ok) {
+		atomicAdd(&res->frame_ok, 1ull);
+	} else {
+		atomicAdd(&res->frame_miss, 1ull);
+		atomicMin(&res->first_miss, (unsigned long long)idx);
+	}
+}
+
 // One thread per record.  `isums` are the input's K1 sums (body from byte 280), `orecs`/`osums`
 // the output records and their payload sums in the re-encoding modes (null in VERIFY).  Record r
-// is record `base + r` of the stream.
+// is record `base + r` of the stream.  With `sha256` (MTZ_FLAG_BLOCK_SHA256) the sha256 keys this
+// stage can check are left to k_block_sha256 instead of being counted as skipped.
 #define BLK_THREADS 128
 __global__ void __launch_bounds__(BLK_THREADS)
 k_block_check(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs,
     const RecSums *__restrict__ isums, const mtz_rec *__restrict__ orecs,
     const RecSums *__restrict__ osums, uint32_t n, uint32_t mode, uint64_t base,
-    BlockResult *__restrict__ res)
+    BlockResult *__restrict__ res, bool sha256)
 {
 	const uint32_t r = blockIdx.x * BLK_THREADS + threadIdx.x;
 	if (r >= n) return;
 	const mtz_rec rec = recs[r];
 	if (rec.type != DRR_WRITE_T) return;
 	const uint8_t *hdr = d_in + rec.off;
-	const uint64_t prop = *reinterpret_cast<const uint64_t *>(hdr + 88);
-	const uint64_t lsz = ((prop & 0xffffull) + 1ull) * 512ull;
-	const uint64_t psz = (((prop >> 16) & 0xffffull) + 1ull) * 512ull;
-	const uint32_t dc = (uint32_t)((prop >> 32) & 0x7full);
-	const bool raw_in = rec.comp == 0u, lz4_in = rec.comp == ZIO_LZ4;
-	const bool encodes = mode == MTZ_MODE_COMPRESS || mode == MTZ_MODE_RECOMPRESS;
-	// 0 skipped, 1 logical bytes, 2 disk frame;  src 0 input payload, 1 output payload
-	int what = 0, src = 0;
-	if (hdr[48] == ZIO_CKSUM_FLETCHER4 && prop != 0ull && !((prop >> 39) & 1ull) && lsz == rec.lsize) {
-		if ((dc == BLK_DC_INHERIT || dc == BLK_DC_OFF) && psz == lsz) {
-			if (raw_in) { what = 1; src = 0; }
-			else if (lz4_in && mode == MTZ_MODE_DECOMPRESS && osums != nullptr) { what = 1; src = 1; }
-		} else if (dc == BLK_DC_LZ4) {
-			if (lz4_in) { what = 2; src = 0; }
-			else if (raw_in && encodes && osums != nullptr) { what = 2; src = 1; }
-		}
+	const BlockClass c = block_classify(hdr, rec, mode, osums != nullptr, ZIO_CKSUM_FLETCHER4);
+	const int what = c.what, src = c.src;
+	if (what == 0) {
+		if (!sha256 || block_classify(hdr, rec, mode, osums != nullptr, ZIO_CKSUM_SHA256).what == 0)
+			atomicAdd(&res->skipped, 1ull);
+		return;
 	}
-	if (what == 0) { atomicAdd(&res->skipped, 1ull); return; }
 	Ck4 sums;
 	uint64_t nbytes;
 	bool ok = true;
@@ -87,18 +125,10 @@ k_block_check(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs
 		// the stage's encoder stored the block raw where ZFS's stored a frame: not that encoder
 		if (what == 2 && o.comp != ZIO_LZ4) ok = false;
 	}
-	const uint64_t cover = (what == 1) ? lsz : psz;
+	const uint64_t cover = (what == 1) ? c.lsz : c.psz;
 	if (nbytes > cover) ok = false;
 	if (ok) ok = ck_eq(shift_zeros(sums, (cover - nbytes) >> 2), load_ck(hdr + 56));
-	if (what == 1) {
-		if (ok) atomicAdd(&res->logical_ok, 1ull);
-		else atomicMin(&res->first_bad, (unsigned long long)(base + r));
-	} else if (ok) {
-		atomicAdd(&res->frame_ok, 1ull);
-	} else {
-		atomicAdd(&res->frame_miss, 1ull);
-		atomicMin(&res->first_miss, (unsigned long long)(base + r));
-	}
+	block_verdict(res, what, ok, base + r);
 }
 
 } // namespace mtz

@@ -15,6 +15,7 @@
 #include "kernels_codec.cuh"
 #include "kernels_index.cuh"
 #include "kernels_block.cuh"
+#include "kernels_sha256.cuh"
 
 namespace mtz {
 
@@ -23,12 +24,14 @@ namespace mtz {
 struct BlockPending {
 	BlockResult r;
 	uint64_t obj = 0, off = 0;    // drr_object / drr_offset of record r.first_bad
+	uint8_t ctype = 0;            // ... and its drr_checksumtype
 	BlockPending() { clear(); }
 	void clear()
 	{
-		r.logical_ok = r.frame_ok = r.frame_miss = r.skipped = 0;
+		r.logical_ok = r.frame_ok = r.frame_miss = r.skipped = r.sha256 = 0;
 		r.first_bad = r.first_miss = ~0ull;
 		obj = off = 0;
+		ctype = 0;
 	}
 };
 

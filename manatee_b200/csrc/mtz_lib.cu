@@ -302,6 +302,8 @@ int32_t mtz_open(const mtz_config *cfg, mtz_handle **out)
 		    "one-GPU-per-process shard form");
 	if ((full.flags & MTZ_FLAG_BLOCK_CKSUM) && full.mode == MTZ_MODE_PASSTHROUGH)
 		return fail(nullptr, MTZ_EINVAL, "PASSTHROUGH parses no record: BLOCK_CKSUM needs another mode");
+	if ((full.flags & MTZ_FLAG_BLOCK_SHA256) && !(full.flags & MTZ_FLAG_BLOCK_CKSUM))
+		return fail(nullptr, MTZ_EINVAL, "BLOCK_SHA256 extends the block check: it needs BLOCK_CKSUM");
 	const cudaDeviceProp &prop = props[0];
 
 	mtz_handle *h = new (std::nothrow) mtz_handle();
@@ -546,6 +548,7 @@ static int32_t launch_scan(mtz_handle *h, cudaStream_t st, const RecSums *d_sums
 
 // ------------------------------------------------- block checksums (drr_key) --
 static bool block_on(const mtz_handle *h) { return (h->cfg.flags & MTZ_FLAG_BLOCK_CKSUM) != 0; }
+static bool block_sha256_on(const mtz_handle *h) { return (h->cfg.flags & MTZ_FLAG_BLOCK_SHA256) != 0; }
 
 static int32_t block_reset(mtz_handle *h, cudaStream_t st, BlockResult *bres)
 {
@@ -554,17 +557,26 @@ static int32_t block_reset(mtz_handle *h, cudaStream_t st, BlockResult *bres)
 	return MTZ_OK;
 }
 
-// k_block_check over records [0, nrec) of a (sub-)batch, record 0 being stream record `base`.  Not
-// counted in mtz_stats.kernel_launches: the flag leaves every mtz_stats field as it is.
+// k_block_check over records [0, nrec) of a (sub-)batch, record 0 being stream record `base`, then
+// with MTZ_FLAG_BLOCK_SHA256 k_block_sha256 over the same records (`d_out` = the output batch the
+// offsets of `orecs` refer to; null with `orecs`).  Not counted in mtz_stats.kernel_launches: the
+// flags leave every mtz_stats field as it is.
 static int32_t launch_block(mtz_handle *h, cudaStream_t st, const uint8_t *d_in, const mtz_rec *d_recs,
-    const RecSums *isums, const mtz_rec *orecs, const RecSums *osums, size_t nrec, uint64_t base,
-    BlockResult *bres)
+    const RecSums *isums, const mtz_rec *orecs, const RecSums *osums, const uint8_t *d_out, size_t nrec,
+    uint64_t base, BlockResult *bres)
 {
 	if (nrec == 0) return MTZ_OK;
+	const bool sha = block_sha256_on(h);
 	const unsigned grid = (unsigned)((nrec + BLK_THREADS - 1) / BLK_THREADS);
 	k_block_check<<<grid, BLK_THREADS, 0, st>>>(d_in, d_recs, isums, orecs, osums, (uint32_t)nrec,
-	    h->cfg.mode, base, bres);
+	    h->cfg.mode, base, bres, sha);
 	MTZ_CU(h, cudaGetLastError());
+	if (sha) {
+		const unsigned gs = (unsigned)((nrec + SHA_THREADS - 1) / SHA_THREADS);
+		k_block_sha256<<<gs, SHA_THREADS, 0, st>>>(d_in, d_recs, d_out, orecs, (uint32_t)nrec, h->cfg.mode,
+		    base, bres);
+		MTZ_CU(h, cudaGetLastError());
+	}
 	return MTZ_OK;
 }
 
@@ -575,13 +587,13 @@ static int32_t block_take(mtz_handle *h, BlockPending &p, const BlockResult &r, 
     uint64_t off)
 {
 	p.r.logical_ok += r.logical_ok; p.r.frame_ok += r.frame_ok;
-	p.r.frame_miss += r.frame_miss; p.r.skipped += r.skipped;
+	p.r.frame_miss += r.frame_miss; p.r.skipped += r.skipped; p.r.sha256 += r.sha256;
 	p.r.first_miss = std::min(p.r.first_miss, r.first_miss);
 	if (r.first_bad < p.r.first_bad) {
-		uint64_t w[4];
+		uint64_t w[6];      // header bytes 8..55: drr_object, drr_offset, drr_checksumtype
 		MTZ_CU(h, cudaMemcpy(w, d_in + off + 8, sizeof w, cudaMemcpyDeviceToHost));
 		p.r.first_bad = r.first_bad;
-		p.obj = w[0]; p.off = w[2];
+		p.obj = w[0]; p.off = w[2]; p.ctype = (uint8_t)w[5];
 	}
 	return MTZ_OK;
 }
@@ -597,6 +609,7 @@ static int32_t block_fold(mtz_handle *h, BlockPending &p, uint64_t stream_bad)
 		std::lock_guard<std::mutex> g(h->stats_mu);
 		h->bstats.logical_ok += q.r.logical_ok; h->bstats.frame_ok += q.r.frame_ok;
 		h->bstats.frame_miss += q.r.frame_miss; h->bstats.skipped += q.r.skipped;
+		h->bstats.sha256 += q.r.sha256;
 		h->bstats.first_frame_miss = std::min<uint64_t>(h->bstats.first_frame_miss, q.r.first_miss);
 	}
 	if (q.r.first_bad == ~0ull || q.r.first_bad >= stream_bad) return MTZ_OK;
@@ -605,8 +618,9 @@ static int32_t block_fold(mtz_handle *h, BlockPending &p, uint64_t stream_bad)
 		if (q.r.first_bad < h->stats.bad_record) h->stats.bad_record = q.r.first_bad;
 	}
 	return fail(h, MTZ_ECKSUM, "block checksum mismatch at record %llu (object %llu, offset %llu): "
-	    "the bytes differ from the block on disk", (unsigned long long)q.r.first_bad,
-	    (unsigned long long)q.obj, (unsigned long long)q.off);
+	    "the bytes differ from the block on disk%s", (unsigned long long)q.r.first_bad,
+	    (unsigned long long)q.obj, (unsigned long long)q.off,
+	    q.ctype == ZIO_CKSUM_SHA256 ? " (sha256 key)" : "");
 }
 
 static int32_t ensure_dv_sums(mtz_handle *h, size_t need, cudaStream_t st)
@@ -792,7 +806,7 @@ static int32_t codec_launch_post(mtz_handle *h, cudaStream_t st, CodecBufs &cb, 
 	// output records of a codec batch are smaller than the logical size: decide by the input's
 	launch_k1_kernel(h, st, d_out, orecs, n, osums, 312u, cb.avg_out_rec);
 	if (bres != nullptr) {
-		const int32_t rc = launch_block(h, st, d_in, d_recs, isums, orecs, osums, nrec, bbase, bres);
+		const int32_t rc = launch_block(h, st, d_in, d_recs, isums, orecs, osums, d_out, nrec, bbase, bres);
 		if (rc != MTZ_OK) return rc;
 	}
 	if (all_osums == nullptr) {
@@ -860,8 +874,8 @@ int32_t mtz_dev_submit(mtz_handle *h, const void *d_in, size_t in_bytes,
 		h->dv_in = (const uint8_t *)d_in; h->dv_recs = d_recs;
 		rc = block_reset(h, st, h->dv_bres);
 		if (rc == MTZ_OK && !is_codec_mode(h->cfg.mode))
-			rc = launch_block(h, st, (const uint8_t *)d_in, d_recs, h->dv_sums, nullptr, nullptr, nrec,
-			    h->dv_first, h->dv_bres);
+			rc = launch_block(h, st, (const uint8_t *)d_in, d_recs, h->dv_sums, nullptr, nullptr, nullptr,
+			    nrec, h->dv_first, h->dv_bres);
 		if (rc != MTZ_OK) return rc;
 	}
 	if (!is_codec_mode(h->cfg.mode)) return MTZ_OK;
@@ -1439,8 +1453,8 @@ static int32_t submit_batch(mtz_handle *h, Slot &s, const uint8_t *p0, size_t n0
 		if (block_on(h) && nrec > 0) {
 			rc = block_reset(h, s.st, s.d_bres);
 			if (rc == MTZ_OK)
-				rc = launch_block(h, s.st, s.d_in, s.d_recs, h->dv_sums + h->dv_nrec, nullptr, nullptr, nrec,
-				    s.first_rec, s.d_bres);
+				rc = launch_block(h, s.st, s.d_in, s.d_recs, h->dv_sums + h->dv_nrec, nullptr, nullptr, nullptr,
+				    nrec, s.first_rec, s.d_bres);
 			if (rc != MTZ_OK) return rc;
 		}
 		if (h->dv_nrec == 0) h->dv_first = s.first_rec;
@@ -1454,7 +1468,8 @@ static int32_t submit_batch(mtz_handle *h, Slot &s, const uint8_t *p0, size_t n0
 			// VERIFY checks the input here; the codec modes after the output's sums (codec_launch_post)
 			rc = block_reset(h, s.st, s.d_bres);
 			if (rc == MTZ_OK && !is_codec_mode(h->cfg.mode))
-				rc = launch_block(h, s.st, s.d_in, s.d_recs, s.d_sums, nullptr, nullptr, nrec, s.first_rec, s.d_bres);
+				rc = launch_block(h, s.st, s.d_in, s.d_recs, s.d_sums, nullptr, nullptr, nullptr, nrec, s.first_rec,
+				    s.d_bres);
 			if (rc != MTZ_OK) return rc;
 		}
 		if (is_codec_mode(h->cfg.mode)) {

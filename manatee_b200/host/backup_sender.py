@@ -131,7 +131,8 @@ class BackupSender(object):
         return GpuSnapshotStage(g["mode"], device=g.get("device", 0), devices=g.get("devices"),
                                 ring_bytes=g.get("ringBytes", 0), batch_bytes=g.get("batchBytes", 0),
                                 out_ring_bytes=g.get("outRingBytes", 0), n_slots=g.get("slots", 0),
-                                block_checksums=bool(g.get("blockChecksums")))
+                                block_checksums=bool(g.get("blockChecksums")),
+                                block_sha256=bool(g.get("blockSha256")))
 
     def _stage_stats(self, stage):
         """job.gpu: the stage counters, plus `blocks` (block-checksum counters) with
