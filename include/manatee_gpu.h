@@ -75,6 +75,12 @@ extern "C" {
                                   * by the same rules and with the same consequences as fletcher4 keys;
                                   * mtz_block_stats.sha256 counts them.  Without this flag they are skipped */
 
+#define MTZ_FLAG_BLOCK_SHA512 16u /* with MTZ_FLAG_BLOCK_CKSUM only (MTZ_EINVAL without it), independent of
+                                  * MTZ_FLAG_BLOCK_SHA256: also check the records whose key is a SHA-512/256
+                                  * (drr_checksumtype 11, checksum=sha512), by the same rules and with the
+                                  * same consequences as fletcher4 keys; mtz_block_stats.sha512 counts them.
+                                  * Without this flag they are skipped */
+
 typedef struct mtz_handle mtz_handle;
 
 #define MTZ_MAX_DEVICES 16
@@ -122,8 +128,9 @@ typedef struct mtz_stats {
 } mtz_stats;
 
 /* MTZ_FLAG_BLOCK_CKSUM counters (all zero with the flag off).  A DRR_WRITE whose key the stage
- * cannot check (not fletcher4 -- or sha256 with MTZ_FLAG_BLOCK_SHA256 --, no key, encrypted, another
- * on-disk compression, or no bytes at hand that the key covers) counts as skipped. */
+ * cannot check (not fletcher4 -- or sha256 with MTZ_FLAG_BLOCK_SHA256, sha512 with MTZ_FLAG_BLOCK_SHA512 --,
+ * no key, encrypted, another on-disk compression, or no bytes at hand that the key covers) counts as
+ * skipped. */
 typedef struct mtz_block_stats {
 	uint32_t struct_size;       /* sizeof(mtz_block_stats), set by the caller */
 	uint32_t pad;
@@ -134,6 +141,7 @@ typedef struct mtz_block_stats {
 	uint64_t first_frame_miss;  /* stream index of the first frame miss, ~0 if none */
 	uint64_t sha256;            /* MTZ_FLAG_BLOCK_SHA256: records compared by SHA-256 (also counted above,
 	                               or the cause of the failure) */
+	uint64_t sha512;            /* MTZ_FLAG_BLOCK_SHA512: records compared by SHA-512/256 (likewise) */
 } mtz_block_stats;
 
 /* One DRR record as seen by the kernels (32 B, little endian). */

@@ -1,7 +1,8 @@
 // kernels_block.cuh -- block-checksum check (MTZ_FLAG_BLOCK_CKSUM): every DRR_WRITE record
 // against the on-disk block checksum `zfs send` copies into its header ([EXTERNAL] dmu_send.c
 // dump_write(); SURVEY.md App. A.1):
-//   byte 48      drr_checksumtype (7 = fletcher4, 8 = sha256: kernels_sha256.cuh)
+//   byte 48      drr_checksumtype (7 = fletcher4, 8 = sha256: kernels_sha256.cuh,
+//                11 = sha512: kernels_sha512.cuh)
 //   bytes 56..87 drr_key.ddk_cksum, the block pointer's checksum of the PSIZE bytes on disk
 //   bytes 88..95 drr_key.ddk_prop: LSIZE bits 0..15 and PSIZE bits 16..31 as (size/512 - 1),
 //                on-disk compression bits 32..38, crypt bit 39
@@ -17,6 +18,7 @@ namespace mtz {
 
 #define ZIO_CKSUM_FLETCHER4 7u
 #define ZIO_CKSUM_SHA256    8u
+#define ZIO_CKSUM_SHA512    11u
 #define BLK_DC_INHERIT 0u      // "stored raw": the key covers the logical block
 #define BLK_DC_OFF     2u
 #define BLK_DC_LZ4     15u     // the key covers ZFS's LZ4 frame, zero-padded to PSIZE
@@ -24,6 +26,7 @@ namespace mtz {
 struct BlockResult {           // device, mirrored to pinned host; zeroed per batch
 	unsigned long long logical_ok, frame_ok, frame_miss, skipped;
 	unsigned long long sha256;       // records compared by k_block_sha256 (kernels_sha256.cuh)
+	unsigned long long sha512;       // records compared by k_block_sha512 (kernels_sha512.cuh)
 	unsigned long long first_bad;    // stream index of the first logical mismatch, ~0 none
 	unsigned long long first_miss;   // stream index of the first frame mismatch, ~0 none
 };
@@ -89,14 +92,16 @@ __device__ __forceinline__ void block_verdict(BlockResult *res, int what, bool o
 
 // One thread per record.  `isums` are the input's K1 sums (body from byte 280), `orecs`/`osums`
 // the output records and their payload sums in the re-encoding modes (null in VERIFY).  Record r
-// is record `base + r` of the stream.  With `sha256` (MTZ_FLAG_BLOCK_SHA256) the sha256 keys this
-// stage can check are left to k_block_sha256 instead of being counted as skipped.
+// is record `base + r` of the stream.  `hashed` has bit t set for each key type t another kernel
+// hashes (bit 8: k_block_sha256 with MTZ_FLAG_BLOCK_SHA256, bit 11: k_block_sha512 with
+// MTZ_FLAG_BLOCK_SHA512): the keys of those types this stage can check are left to that kernel
+// instead of being counted as skipped.
 #define BLK_THREADS 128
 __global__ void __launch_bounds__(BLK_THREADS)
 k_block_check(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs,
     const RecSums *__restrict__ isums, const mtz_rec *__restrict__ orecs,
     const RecSums *__restrict__ osums, uint32_t n, uint32_t mode, uint64_t base,
-    BlockResult *__restrict__ res, bool sha256)
+    BlockResult *__restrict__ res, uint32_t hashed)
 {
 	const uint32_t r = blockIdx.x * BLK_THREADS + threadIdx.x;
 	if (r >= n) return;
@@ -106,7 +111,8 @@ k_block_check(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs
 	const BlockClass c = block_classify(hdr, rec, mode, osums != nullptr, ZIO_CKSUM_FLETCHER4);
 	const int what = c.what, src = c.src;
 	if (what == 0) {
-		if (!sha256 || block_classify(hdr, rec, mode, osums != nullptr, ZIO_CKSUM_SHA256).what == 0)
+		const uint32_t t = hdr[48];
+		if (t >= 32u || !((hashed >> t) & 1u) || block_classify(hdr, rec, mode, osums != nullptr, t).what == 0)
 			atomicAdd(&res->skipped, 1ull);
 		return;
 	}

@@ -16,6 +16,7 @@
 #include "kernels_index.cuh"
 #include "kernels_block.cuh"
 #include "kernels_sha256.cuh"
+#include "kernels_sha512.cuh"
 
 namespace mtz {
 
@@ -28,7 +29,7 @@ struct BlockPending {
 	BlockPending() { clear(); }
 	void clear()
 	{
-		r.logical_ok = r.frame_ok = r.frame_miss = r.skipped = r.sha256 = 0;
+		r.logical_ok = r.frame_ok = r.frame_miss = r.skipped = r.sha256 = r.sha512 = 0;
 		r.first_bad = r.first_miss = ~0ull;
 		obj = off = 0;
 		ctype = 0;

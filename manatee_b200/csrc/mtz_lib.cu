@@ -304,6 +304,8 @@ int32_t mtz_open(const mtz_config *cfg, mtz_handle **out)
 		return fail(nullptr, MTZ_EINVAL, "PASSTHROUGH parses no record: BLOCK_CKSUM needs another mode");
 	if ((full.flags & MTZ_FLAG_BLOCK_SHA256) && !(full.flags & MTZ_FLAG_BLOCK_CKSUM))
 		return fail(nullptr, MTZ_EINVAL, "BLOCK_SHA256 extends the block check: it needs BLOCK_CKSUM");
+	if ((full.flags & MTZ_FLAG_BLOCK_SHA512) && !(full.flags & MTZ_FLAG_BLOCK_CKSUM))
+		return fail(nullptr, MTZ_EINVAL, "BLOCK_SHA512 extends the block check: it needs BLOCK_CKSUM");
 	const cudaDeviceProp &prop = props[0];
 
 	mtz_handle *h = new (std::nothrow) mtz_handle();
@@ -549,6 +551,7 @@ static int32_t launch_scan(mtz_handle *h, cudaStream_t st, const RecSums *d_sums
 // ------------------------------------------------- block checksums (drr_key) --
 static bool block_on(const mtz_handle *h) { return (h->cfg.flags & MTZ_FLAG_BLOCK_CKSUM) != 0; }
 static bool block_sha256_on(const mtz_handle *h) { return (h->cfg.flags & MTZ_FLAG_BLOCK_SHA256) != 0; }
+static bool block_sha512_on(const mtz_handle *h) { return (h->cfg.flags & MTZ_FLAG_BLOCK_SHA512) != 0; }
 
 static int32_t block_reset(mtz_handle *h, cudaStream_t st, BlockResult *bres)
 {
@@ -558,22 +561,29 @@ static int32_t block_reset(mtz_handle *h, cudaStream_t st, BlockResult *bres)
 }
 
 // k_block_check over records [0, nrec) of a (sub-)batch, record 0 being stream record `base`, then
-// with MTZ_FLAG_BLOCK_SHA256 k_block_sha256 over the same records (`d_out` = the output batch the
-// offsets of `orecs` refer to; null with `orecs`).  Not counted in mtz_stats.kernel_launches: the
-// flags leave every mtz_stats field as it is.
+// with MTZ_FLAG_BLOCK_SHA256 k_block_sha256 and with MTZ_FLAG_BLOCK_SHA512 k_block_sha512 over the
+// same records (`d_out` = the output batch the offsets of `orecs` refer to; null with `orecs`).  Not
+// counted in mtz_stats.kernel_launches: the flags leave every mtz_stats field as it is.
 static int32_t launch_block(mtz_handle *h, cudaStream_t st, const uint8_t *d_in, const mtz_rec *d_recs,
     const RecSums *isums, const mtz_rec *orecs, const RecSums *osums, const uint8_t *d_out, size_t nrec,
     uint64_t base, BlockResult *bres)
 {
 	if (nrec == 0) return MTZ_OK;
-	const bool sha = block_sha256_on(h);
+	const bool sha = block_sha256_on(h), sha512 = block_sha512_on(h);
+	const uint32_t hashed = (sha ? 1u << ZIO_CKSUM_SHA256 : 0u) | (sha512 ? 1u << ZIO_CKSUM_SHA512 : 0u);
 	const unsigned grid = (unsigned)((nrec + BLK_THREADS - 1) / BLK_THREADS);
 	k_block_check<<<grid, BLK_THREADS, 0, st>>>(d_in, d_recs, isums, orecs, osums, (uint32_t)nrec,
-	    h->cfg.mode, base, bres, sha);
+	    h->cfg.mode, base, bres, hashed);
 	MTZ_CU(h, cudaGetLastError());
 	if (sha) {
 		const unsigned gs = (unsigned)((nrec + SHA_THREADS - 1) / SHA_THREADS);
 		k_block_sha256<<<gs, SHA_THREADS, 0, st>>>(d_in, d_recs, d_out, orecs, (uint32_t)nrec, h->cfg.mode,
+		    base, bres);
+		MTZ_CU(h, cudaGetLastError());
+	}
+	if (sha512) {
+		const unsigned gs = (unsigned)((nrec + SHA512_THREADS - 1) / SHA512_THREADS);
+		k_block_sha512<<<gs, SHA512_THREADS, 0, st>>>(d_in, d_recs, d_out, orecs, (uint32_t)nrec, h->cfg.mode,
 		    base, bres);
 		MTZ_CU(h, cudaGetLastError());
 	}
@@ -588,6 +598,7 @@ static int32_t block_take(mtz_handle *h, BlockPending &p, const BlockResult &r, 
 {
 	p.r.logical_ok += r.logical_ok; p.r.frame_ok += r.frame_ok;
 	p.r.frame_miss += r.frame_miss; p.r.skipped += r.skipped; p.r.sha256 += r.sha256;
+	p.r.sha512 += r.sha512;
 	p.r.first_miss = std::min(p.r.first_miss, r.first_miss);
 	if (r.first_bad < p.r.first_bad) {
 		uint64_t w[6];      // header bytes 8..55: drr_object, drr_offset, drr_checksumtype
@@ -609,7 +620,7 @@ static int32_t block_fold(mtz_handle *h, BlockPending &p, uint64_t stream_bad)
 		std::lock_guard<std::mutex> g(h->stats_mu);
 		h->bstats.logical_ok += q.r.logical_ok; h->bstats.frame_ok += q.r.frame_ok;
 		h->bstats.frame_miss += q.r.frame_miss; h->bstats.skipped += q.r.skipped;
-		h->bstats.sha256 += q.r.sha256;
+		h->bstats.sha256 += q.r.sha256; h->bstats.sha512 += q.r.sha512;
 		h->bstats.first_frame_miss = std::min<uint64_t>(h->bstats.first_frame_miss, q.r.first_miss);
 	}
 	if (q.r.first_bad == ~0ull || q.r.first_bad >= stream_bad) return MTZ_OK;
@@ -620,7 +631,7 @@ static int32_t block_fold(mtz_handle *h, BlockPending &p, uint64_t stream_bad)
 	return fail(h, MTZ_ECKSUM, "block checksum mismatch at record %llu (object %llu, offset %llu): "
 	    "the bytes differ from the block on disk%s", (unsigned long long)q.r.first_bad,
 	    (unsigned long long)q.obj, (unsigned long long)q.off,
-	    q.ctype == ZIO_CKSUM_SHA256 ? " (sha256 key)" : "");
+	    q.ctype == ZIO_CKSUM_SHA256 ? " (sha256 key)" : q.ctype == ZIO_CKSUM_SHA512 ? " (sha512 key)" : "");
 }
 
 static int32_t ensure_dv_sums(mtz_handle *h, size_t need, cudaStream_t st)

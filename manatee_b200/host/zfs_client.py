@@ -121,7 +121,8 @@ class ZfsClient(object):
                                 ring_bytes=g.get("ringBytes", 0), batch_bytes=g.get("batchBytes", 0),
                                 out_ring_bytes=g.get("outRingBytes", 0), n_slots=g.get("slots", 0),
                                 block_checksums=bool(g.get("blockChecksums")),
-                                block_sha256=bool(g.get("blockSha256")))
+                                block_sha256=bool(g.get("blockSha256")),
+                                block_sha512=bool(g.get("blockSha512")))
 
     def _wire_mode(self, serverUrl, jobPath):
         """Which stage to put in the pipe for THIS job (SURVEY.md 8f f2).  A receiver configured

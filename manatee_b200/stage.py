@@ -20,17 +20,22 @@ class GpuSnapshotStage(object):
     """One stage instance == one mtz_handle == one stream (like one Transform)."""
 
     def __init__(self, mode="verify", device=0, ring_bytes=0, batch_bytes=0, n_slots=0,
-                 out_ring_bytes=0, flags=0, devices=None, block_checksums=False, block_sha256=False):
+                 out_ring_bytes=0, flags=0, devices=None, block_checksums=False, block_sha256=False,
+                 block_sha512=False):
         """``devices`` = CUDA ordinals of a device group: the GPUs of one box run as ONE stage,
         batch b of the stream on ``devices[b % len(devices)]`` (mtz_config.devices[]).
         ``block_checksums`` = MTZ_FLAG_BLOCK_CKSUM: every DRR_WRITE is also checked against the
         on-disk block checksum the stream carries (``block_stats()``).
         ``block_sha256`` = MTZ_FLAG_BLOCK_SHA256: the check also covers SHA-256 keys
-        (checksum=sha256); only valid with ``block_checksums``, MtzError(EINVAL) otherwise."""
+        (checksum=sha256); only valid with ``block_checksums``, MtzError(EINVAL) otherwise.
+        ``block_sha512`` = MTZ_FLAG_BLOCK_SHA512: likewise for SHA-512/256 keys (checksum=sha512),
+        with or without ``block_sha256``."""
         if block_checksums:
             flags |= N.FLAG_BLOCK_CKSUM
         if block_sha256:
             flags |= N.FLAG_BLOCK_SHA256
+        if block_sha512:
+            flags |= N.FLAG_BLOCK_SHA512
         self._L = N.lib()
         self._h = C.c_void_p()
         cfg = N.Config()

@@ -12,6 +12,8 @@ that both see the same machine:
   recompress  the `zfs send -c` form of a resident 1 GiB stream whose SHA-256 keys say "written with
               compression=lz4": the kernel runs on the post stream ahead of the stamp chain
 
+tools/block_sha512_cost.py runs the same legs for MTZ_FLAG_BLOCK_SHA512 (main("sha512")).
+
 Prints one JSON line (and writes it to --out) with the GPU name and power limit the numbers were
 taken on.
 usage: tools/block_sha256_cost.py [--verify-gib 16] [--host-gib 2] [--recompress-gib 1] [--steps 10]
@@ -29,12 +31,16 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 from block_cksum_cost import gpu_info  # noqa: E402
 
+# the hash a run measures: its leg is the flag on top of MTZ_FLAG_BLOCK_CKSUM; `block` = the bytes of
+# one compression block (a message of a 128 KiB record hashes 128 KiB + one padding block)
+HASHES = {"sha256": {"kernel": "k_block_sha256", "block": 64},
+          "sha512": {"kernel": "k_block_sha512", "block": 128}}
 LEGS = ("cksum", "sha256")
 
 
 def _stage(mode, leg):
     from manatee_b200 import GpuSnapshotStage
-    return GpuSnapshotStage(mode, block_checksums=True, block_sha256=(leg == "sha256"))
+    return GpuSnapshotStage(mode, block_checksums=True, **({"block_" + leg: True} if leg in HASHES else {}))
 
 
 def _summary(ms):
@@ -45,13 +51,13 @@ def _summary(ms):
         res[name + "_ms_median"] = v[len(v) // 2]
         res[name + "_ms_min"] = v[0]
         res[name + "_ms_max"] = v[-1]
-    res["diff_ms_mean"] = res["sha256_ms_mean"] - res["cksum_ms_mean"]
+    res["diff_ms_mean"] = res[LEGS[1] + "_ms_mean"] - res["cksum_ms_mean"]
     res["diff_pct_mean"] = 100.0 * res["diff_ms_mean"] / res["cksum_ms_mean"]
     return res
 
 
 def resident_legs(mode, s, steps, warm, out_cap, profile_steps=0):
-    """mean ms per resident step (dev_submit + dev_finish), BLOCK_CKSUM vs BLOCK_CKSUM|BLOCK_SHA256"""
+    """mean ms per resident step (dev_submit + dev_finish), BLOCK_CKSUM vs BLOCK_CKSUM|the hash's flag"""
     import numpy as np
     import torch
     from manatee_b200 import index_host
@@ -86,13 +92,13 @@ def resident_legs(mode, s, steps, warm, out_cap, profile_steps=0):
                 if i == warm + steps - 1 and d_out is not None:
                     outs[name] = (ob, d_out[:ob].view(torch.int64).sum().item())    # records are 8-byte aligned
         res = _summary(ms)
-        res["block_stats"] = legs["sha256"].block_stats()
+        res["block_stats"] = legs[LEGS[1]].block_stats()
         res["records"] = int(len(recs))
         res["stream_bytes"] = int(s.size)
         if outs:
-            res["outputs_equal"] = outs["cksum"] == outs["sha256"]
+            res["outputs_equal"] = outs["cksum"] == outs[LEGS[1]]
         if profile_steps:
-            res.update(kernel_time(lambda: step(legs["sha256"]), profile_steps))
+            res.update(kernel_time(lambda: step(legs[LEGS[1]]), profile_steps))
         return res
     finally:
         for g in legs.values():
@@ -100,7 +106,7 @@ def resident_legs(mode, s, steps, warm, out_cap, profile_steps=0):
 
 
 def kernel_time(fn, n):
-    """device time per step of k_block_sha256 (torch.profiler, CUDA activities), over n steps"""
+    """device time per step of the hash kernel (torch.profiler, CUDA activities), over n steps"""
     import torch
     from torch.profiler import ProfilerActivity, profile
     torch.cuda.synchronize()
@@ -108,12 +114,13 @@ def kernel_time(fn, n):
         for _ in range(n):
             fn()
         torch.cuda.synchronize()
+    kern = HASHES[LEGS[1]]["kernel"]
     us, calls = 0.0, 0
     for e in prof.key_averages():
-        if "k_block_sha256" in e.key:
+        if kern in e.key:
             us += getattr(e, "device_time_total", None) or getattr(e, "cuda_time_total", 0.0)
             calls += e.count
-    return {"k_block_sha256_ms_per_step": us / 1000.0 / n, "k_block_sha256_launches_per_step": calls / n}
+    return {kern + "_ms_per_step": us / 1000.0 / n, kern + "_launches_per_step": calls / n}
 
 
 def host_legs(s, steps, warm):
@@ -132,7 +139,7 @@ def host_legs(s, steps, warm):
         res = _summary(ms)
         for name in LEGS:
             res[name + "_gbps"] = s.size / (res[name + "_ms_mean"] * 1e6)
-        res["block_stats"] = legs["sha256"].block_stats()
+        res["block_stats"] = legs[LEGS[1]].block_stats()
         res["stream_bytes"] = int(s.size)
         return res
     finally:
@@ -140,7 +147,10 @@ def host_legs(s, steps, warm):
             g.close()
 
 
-def main():
+def main(hash_name="sha256"):
+    global LEGS
+    LEGS = ("cksum", hash_name)
+    kern, blk = HASHES[hash_name]["kernel"], HASHES[hash_name]["block"]
     ap = argparse.ArgumentParser()
     ap.add_argument("--verify-gib", type=float, default=16.0)
     ap.add_argument("--host-gib", type=float, default=2.0)
@@ -153,28 +163,29 @@ def main():
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
-        sys.exit("block_sha256_cost.py measures device time: it needs a GPU")
+        sys.exit("block_%s_cost.py measures device time: it needs a GPU" % hash_name)
     import oracle as O
-    import block_sha256_ref as R
+    import block_sha512_ref as R
     O.build()
     nth = os.cpu_count() or 1
-    result = {"tool": "block_sha256_cost", **gpu_info(), "steps": args.steps, "warmup": args.warmup}
+    rekey = R.as_sha256 if hash_name == "sha256" else R.as_sha512
+    result = {"tool": "block_%s_cost" % hash_name, **gpu_info(), "steps": args.steps, "warmup": args.warmup}
 
     rs = 131072
     n = max(1, int(args.verify_gib * (1 << 30)) // (rs + 312))
-    s = R.as_sha256(O, O.synth_stream(n, rs, O.PAYLOAD_PCG, nthreads=nth), threads=nth)
+    s = rekey(O, O.synth_stream(n, rs, O.PAYLOAD_PCG, nthreads=nth), threads=nth)
     v = resident_legs("verify", s, args.steps, args.warmup, 0, args.profile_steps)
-    hashed = v["block_stats"]["sha256"] // (args.steps + args.warmup) * (rs + 64)
+    hashed = v["block_stats"][hash_name] // (args.steps + args.warmup) * (rs + blk)
     v["hashed_bytes_per_step"] = hashed
-    if v.get("k_block_sha256_ms_per_step"):
-        v["k_block_sha256_gbps"] = hashed / (v["k_block_sha256_ms_per_step"] * 1e6)
+    if v.get(kern + "_ms_per_step"):
+        v[kern + "_gbps"] = hashed / (v[kern + "_ms_per_step"] * 1e6)
     result["verify"] = v
     del s
 
     result["host"] = {}
     for rs in (131072, 1 << 20):
         n = max(1, int(args.host_gib * (1 << 30)) // (rs + 312))
-        s = R.as_sha256(O, O.synth_stream(n, rs, O.PAYLOAD_PCG, nthreads=nth), threads=nth)
+        s = rekey(O, O.synth_stream(n, rs, O.PAYLOAD_PCG, nthreads=nth), threads=nth)
         result["host"]["recsize_%d" % rs] = host_legs(s, args.host_steps, 1)
         del s
 
@@ -182,7 +193,7 @@ def main():
     n = max(1, int(args.recompress_gib * (1 << 30)) // (rs + 312))
     raw = O.synth_stream(n, rs, O.PAYLOAD_PGPAGE, nthreads=nth)
     disk, _ = R.as_lz4_on_disk(O, raw)
-    c = R.as_send_c(O, R.as_sha256(O, disk, threads=nth))
+    c = R.as_send_c(O, rekey(O, disk, threads=nth))
     result["recompress"] = resident_legs("recompress", c, args.steps, args.warmup, raw.size + (1 << 20),
                                          args.profile_steps)
     line = json.dumps(result)

@@ -34,6 +34,9 @@ PARAMS = {
     "test_ring_api": [(4093,), (1 << 20,)],
     "test_lz4_on_disk_sha256_keys": [(9,), (12,)],
     "test_record_sizes": [(512,), (8192,), (131072,), (1 << 20,)],
+    "test_lz4_on_disk_sha512_keys": [(9,), (12,)],
+    "test_one_stream_mixing_fletcher4_sha256_sha512_and_skipped_keys": [(False, False), (True, False),
+                                                                        (False, True), (True, True)],
 }
 SKIP = {"test_sixteen_mib_record": "16 MiB blocks take minutes per encode on the emulator",
         "test_size_independent_properties_at_2gib": "2 GiB of LZ4 work is out of reach for the emulator",
@@ -54,12 +57,13 @@ def main():
     N.SO_PATH, N._lib = so, None
     import test_gpu_block_cksum as B
     import test_gpu_block_sha256 as H
+    import test_gpu_block_sha512 as W
     import test_gpu_codec as K
     import test_gpu_lz4 as Z
     import test_gpu_stream as S
     import test_gpu_verify as V
     tot = fail = 0
-    for mod in (V, S, Z, K, B, H):
+    for mod in (V, S, Z, K, B, H, W):
         for name, fn in inspect.getmembers(mod, inspect.isfunction):
             if not name.startswith("test_") or filt not in name:
                 continue
