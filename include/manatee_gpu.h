@@ -81,6 +81,15 @@ extern "C" {
                                   * same consequences as fletcher4 keys; mtz_block_stats.sha512 counts them.
                                   * Without this flag they are skipped */
 
+#define MTZ_FLAG_BLOCK_FRAMES 32u /* with MTZ_FLAG_BLOCK_CKSUM only (MTZ_EINVAL without it), with or without the
+                                  * SHA flags.  VERIFY: a DRR_WRITE that arrives raw while its key covers an
+                                  * LZ4 frame on disk (otherwise skipped) gets a frame from the stage's
+                                  * encoder, compared with the key by the rules COMPRESS applies to its own
+                                  * output: frame_ok, or frame_miss (counted, never an error).  The output
+                                  * bytes do not change.  mtz_block_stats.frames_encoded counts these
+                                  * frames; with this flag and batch_bytes 0 VERIFY batches are 256 MiB.
+                                  * The other modes accept the flag and do not change */
+
 typedef struct mtz_handle mtz_handle;
 
 #define MTZ_MAX_DEVICES 16
@@ -93,7 +102,8 @@ typedef struct mtz_config {
 	uint32_t flags;         /* MTZ_FLAG_* */
 	uint64_t ring_bytes;    /* pinned input ring (0 = max(256 MiB, 2 x batch_bytes)) */
 	uint64_t out_ring_bytes;/* pinned output ring, codec modes (0 = ring_bytes) */
-	uint64_t batch_bytes;   /* target bytes per GPU batch (0 = 32 MiB; 256 MiB in codec modes) */
+	uint64_t batch_bytes;   /* target bytes per GPU batch (0 = 32 MiB; 256 MiB in codec modes and
+	                         * with MTZ_FLAG_BLOCK_FRAMES) */
 	uint32_t record_bytes;  /* expected recordsize hint (0 = 131072) */
 	uint32_t n_slots;       /* batches in flight PER DEVICE (0 = 4) */
 	/* ---- ABI v2: the GPUs of one box as ONE stage.  The stream is cut into whole-record
@@ -142,6 +152,8 @@ typedef struct mtz_block_stats {
 	uint64_t sha256;            /* MTZ_FLAG_BLOCK_SHA256: records compared by SHA-256 (also counted above,
 	                               or the cause of the failure) */
 	uint64_t sha512;            /* MTZ_FLAG_BLOCK_SHA512: records compared by SHA-512/256 (likewise) */
+	uint64_t frames_encoded;    /* MTZ_FLAG_BLOCK_FRAMES: frames encoded for the check (also counted in
+	                               frame_ok / frame_miss, and in sha256 / sha512 where those hashed it) */
 } mtz_block_stats;
 
 /* One DRR record as seen by the kernels (32 B, little endian). */

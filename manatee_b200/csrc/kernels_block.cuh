@@ -27,6 +27,7 @@ struct BlockResult {           // device, mirrored to pinned host; zeroed per ba
 	unsigned long long logical_ok, frame_ok, frame_miss, skipped;
 	unsigned long long sha256;       // records compared by k_block_sha256 (kernels_sha256.cuh)
 	unsigned long long sha512;       // records compared by k_block_sha512 (kernels_sha512.cuh)
+	unsigned long long frames;       // frames encoded for the check (k_frame_sums, kernels_frames.cuh)
 	unsigned long long first_bad;    // stream index of the first logical mismatch, ~0 none
 	unsigned long long first_miss;   // stream index of the first frame mismatch, ~0 none
 };
@@ -46,15 +47,17 @@ __host__ __device__ __forceinline__ Ck4 strip_head8(const Ck4 &whole, const Ck4 
 
 // What a record's key lets the stage compare, decided from its header alone, for keys of type
 // `ctype`: `what` 0 skipped, 1 the logical block, 2 the disk frame; `src` 0 the input payload, 1 the
-// output payload.  `have_out` = the output records of a re-encoding mode are at hand.  Every key
-// type that is checked goes through this one table.
+// output payload, or in VERIFY the frame the declared encoder made of the input (kernels_frames.cuh).
+// `have_out` = the output records of a re-encoding mode are at hand; `frames` = VERIFY with
+// MTZ_FLAG_BLOCK_FRAMES: the encoder's frames of the raw records are.  Every key type that is
+// checked goes through this one table.
 struct BlockClass {
 	int what, src;
 	uint64_t lsz, psz;
 };
 
 __device__ __forceinline__ BlockClass block_classify(const uint8_t *hdr, const mtz_rec &rec, uint32_t mode,
-    bool have_out, uint32_t ctype)
+    bool have_out, uint32_t ctype, bool frames = false)
 {
 	const uint64_t prop = *reinterpret_cast<const uint64_t *>(hdr + 88);
 	BlockClass c;
@@ -70,7 +73,7 @@ __device__ __forceinline__ BlockClass block_classify(const uint8_t *hdr, const m
 			else if (lz4_in && mode == MTZ_MODE_DECOMPRESS && have_out) { c.what = 1; c.src = 1; }
 		} else if (dc == BLK_DC_LZ4) {
 			if (lz4_in) { c.what = 2; c.src = 0; }
-			else if (raw_in && encodes && have_out) { c.what = 2; c.src = 1; }
+			else if (raw_in && ((encodes && have_out) || (frames && mode == MTZ_MODE_VERIFY))) { c.what = 2; c.src = 1; }
 		}
 	}
 	return c;
@@ -95,24 +98,27 @@ __device__ __forceinline__ void block_verdict(BlockResult *res, int what, bool o
 // is record `base + r` of the stream.  `hashed` has bit t set for each key type t another kernel
 // hashes (bit 8: k_block_sha256 with MTZ_FLAG_BLOCK_SHA256, bit 11: k_block_sha512 with
 // MTZ_FLAG_BLOCK_SHA512): the keys of those types this stage can check are left to that kernel
-// instead of being counted as skipped.
+// instead of being counted as skipped.  `fjobs` (VERIFY with MTZ_FLAG_BLOCK_FRAMES, else null): the
+// K3 jobs of kernels_frames.cuh, whose frames stand in for the output records and whose sums are in
+// `osums`.
 #define BLK_THREADS 128
 __global__ void __launch_bounds__(BLK_THREADS)
 k_block_check(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs,
     const RecSums *__restrict__ isums, const mtz_rec *__restrict__ orecs,
     const RecSums *__restrict__ osums, uint32_t n, uint32_t mode, uint64_t base,
-    BlockResult *__restrict__ res, uint32_t hashed)
+    BlockResult *__restrict__ res, uint32_t hashed, const mtz_job *__restrict__ fjobs = nullptr)
 {
 	const uint32_t r = blockIdx.x * BLK_THREADS + threadIdx.x;
 	if (r >= n) return;
 	const mtz_rec rec = recs[r];
 	if (rec.type != DRR_WRITE_T) return;
 	const uint8_t *hdr = d_in + rec.off;
-	const BlockClass c = block_classify(hdr, rec, mode, osums != nullptr, ZIO_CKSUM_FLETCHER4);
+	const bool frames = fjobs != nullptr;
+	const BlockClass c = block_classify(hdr, rec, mode, osums != nullptr, ZIO_CKSUM_FLETCHER4, frames);
 	const int what = c.what, src = c.src;
 	if (what == 0) {
 		const uint32_t t = hdr[48];
-		if (t >= 32u || !((hashed >> t) & 1u) || block_classify(hdr, rec, mode, osums != nullptr, t).what == 0)
+		if (t >= 32u || !((hashed >> t) & 1u) || block_classify(hdr, rec, mode, osums != nullptr, t, frames).what == 0)
 			atomicAdd(&res->skipped, 1ull);
 		return;
 	}
@@ -124,12 +130,17 @@ k_block_check(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs
 		const Ck4 zero = { 0, 0, 0, 0 };
 		nbytes = (uint64_t)rec.payload;
 		sums = strip_head8(s.body, fold_cksum_words(zero, s.emb), s.nbody - 8u);
-	} else {
+	} else if (!frames) {
 		const mtz_rec o = orecs[r];
 		nbytes = (uint64_t)o.payload;
 		sums = osums[r].body;
 		// the stage's encoder stored the block raw where ZFS's stored a frame: not that encoder
 		if (what == 2 && o.comp != ZIO_LZ4) ok = false;
+	} else {
+		const mtz_job j = fjobs[r];
+		nbytes = (uint64_t)j.out_len;
+		sums = osums[r].body;
+		if (j.out_len >= rec.lsize) ok = false;      // stored raw: likewise
 	}
 	const uint64_t cover = (what == 1) ? c.lsz : c.psz;
 	if (nbytes > cover) ok = false;

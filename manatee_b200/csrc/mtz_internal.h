@@ -17,6 +17,7 @@
 #include "kernels_block.cuh"
 #include "kernels_sha256.cuh"
 #include "kernels_sha512.cuh"
+#include "kernels_frames.cuh"
 
 namespace mtz {
 
@@ -29,14 +30,15 @@ struct BlockPending {
 	BlockPending() { clear(); }
 	void clear()
 	{
-		r.logical_ok = r.frame_ok = r.frame_miss = r.skipped = r.sha256 = r.sha512 = 0;
+		r.logical_ok = r.frame_ok = r.frame_miss = r.skipped = r.sha256 = r.sha512 = r.frames = 0;
 		r.first_bad = r.first_miss = ~0ull;
 		obj = off = 0;
 		ctype = 0;
 	}
 };
 
-// device scratch of one codec batch (modes COMPRESS / DECOMPRESS / RECOMPRESS)
+// device scratch of one codec batch (modes COMPRESS / DECOMPRESS / RECOMPRESS); in VERIFY with
+// MTZ_FLAG_BLOCK_FRAMES the encoder's jobs, scratch and frame sums of the block check (enc, d_enc, osums)
 struct CodecBufs {
 	size_t rec_cap = 0, scratch_cap = 0;
 	CodecRec *cr = nullptr;

@@ -306,6 +306,8 @@ int32_t mtz_open(const mtz_config *cfg, mtz_handle **out)
 		return fail(nullptr, MTZ_EINVAL, "BLOCK_SHA256 extends the block check: it needs BLOCK_CKSUM");
 	if ((full.flags & MTZ_FLAG_BLOCK_SHA512) && !(full.flags & MTZ_FLAG_BLOCK_CKSUM))
 		return fail(nullptr, MTZ_EINVAL, "BLOCK_SHA512 extends the block check: it needs BLOCK_CKSUM");
+	if ((full.flags & MTZ_FLAG_BLOCK_FRAMES) && !(full.flags & MTZ_FLAG_BLOCK_CKSUM))
+		return fail(nullptr, MTZ_EINVAL, "BLOCK_FRAMES extends the block check: it needs BLOCK_CKSUM");
 	const cudaDeviceProp &prop = props[0];
 
 	mtz_handle *h = new (std::nothrow) mtz_handle();
@@ -315,8 +317,11 @@ int32_t mtz_open(const mtz_config *cfg, mtz_handle **out)
 	    cfg->mode == MTZ_MODE_RECOMPRESS;
 	// the LZ4 kernels want thousands of records in flight (one warp per record, ~5 ms per
 	// record): measured e2e RECOMPRESS 26 / 41 / 48 / 49 GiB/s logical at 64 / 128 / 256 /
-	// 512 MiB batches; Fletcher alone is happy with 32 MiB batches
-	if (h->cfg.batch_bytes == 0) h->cfg.batch_bytes = codec_mode ? (256ull << 20) : (32ull << 20);
+	// 512 MiB batches; Fletcher alone is happy with 32 MiB batches.  VERIFY with MTZ_FLAG_BLOCK_FRAMES
+	// runs the same encoder over the batch's raw LZ4-keyed records, and wants its records in flight too
+	const bool frames_verify = cfg->mode == MTZ_MODE_VERIFY && (full.flags & MTZ_FLAG_BLOCK_FRAMES);
+	if (h->cfg.batch_bytes == 0)
+		h->cfg.batch_bytes = (codec_mode || frames_verify) ? (256ull << 20) : (32ull << 20);
 	// the input ring holds the batch being filled plus the ones whose H2D copy is still pending
 	if (h->cfg.ring_bytes == 0) h->cfg.ring_bytes = std::max<uint64_t>(256ull << 20, (codec_mode ? 3 : 2) * h->cfg.batch_bytes);
 	if (h->cfg.out_ring_bytes == 0) h->cfg.out_ring_bytes = h->cfg.ring_bytes;
@@ -552,6 +557,16 @@ static int32_t launch_scan(mtz_handle *h, cudaStream_t st, const RecSums *d_sums
 static bool block_on(const mtz_handle *h) { return (h->cfg.flags & MTZ_FLAG_BLOCK_CKSUM) != 0; }
 static bool block_sha256_on(const mtz_handle *h) { return (h->cfg.flags & MTZ_FLAG_BLOCK_SHA256) != 0; }
 static bool block_sha512_on(const mtz_handle *h) { return (h->cfg.flags & MTZ_FLAG_BLOCK_SHA512) != 0; }
+// VERIFY with MTZ_FLAG_BLOCK_FRAMES: the block check encodes frames (kernels_frames.cuh); the other modes
+// accept the flag and have their frames already
+static bool block_frames_on(const mtz_handle *h)
+{
+	return (h->cfg.flags & MTZ_FLAG_BLOCK_FRAMES) != 0 && h->cfg.mode == MTZ_MODE_VERIFY;
+}
+static uint32_t block_hashed(const mtz_handle *h)
+{
+	return (block_sha256_on(h) ? 1u << ZIO_CKSUM_SHA256 : 0u) | (block_sha512_on(h) ? 1u << ZIO_CKSUM_SHA512 : 0u);
+}
 
 static int32_t block_reset(mtz_handle *h, cudaStream_t st, BlockResult *bres)
 {
@@ -562,32 +577,58 @@ static int32_t block_reset(mtz_handle *h, cudaStream_t st, BlockResult *bres)
 
 // k_block_check over records [0, nrec) of a (sub-)batch, record 0 being stream record `base`, then
 // with MTZ_FLAG_BLOCK_SHA256 k_block_sha256 and with MTZ_FLAG_BLOCK_SHA512 k_block_sha512 over the
-// same records (`d_out` = the output batch the offsets of `orecs` refer to; null with `orecs`).  Not
-// counted in mtz_stats.kernel_launches: the flags leave every mtz_stats field as it is.
+// same records (`d_out` = the output batch the offsets of `orecs` refer to; null with `orecs`).
+// `fjobs`: VERIFY's frames (launch_block_frames), with their sums in `osums`.  Not counted in
+// mtz_stats.kernel_launches: the flags leave every mtz_stats field as it is.
 static int32_t launch_block(mtz_handle *h, cudaStream_t st, const uint8_t *d_in, const mtz_rec *d_recs,
     const RecSums *isums, const mtz_rec *orecs, const RecSums *osums, const uint8_t *d_out, size_t nrec,
-    uint64_t base, BlockResult *bres)
+    uint64_t base, BlockResult *bres, const mtz_job *fjobs = nullptr)
 {
 	if (nrec == 0) return MTZ_OK;
 	const bool sha = block_sha256_on(h), sha512 = block_sha512_on(h);
-	const uint32_t hashed = (sha ? 1u << ZIO_CKSUM_SHA256 : 0u) | (sha512 ? 1u << ZIO_CKSUM_SHA512 : 0u);
 	const unsigned grid = (unsigned)((nrec + BLK_THREADS - 1) / BLK_THREADS);
 	k_block_check<<<grid, BLK_THREADS, 0, st>>>(d_in, d_recs, isums, orecs, osums, (uint32_t)nrec,
-	    h->cfg.mode, base, bres, hashed);
+	    h->cfg.mode, base, bres, block_hashed(h), fjobs);
 	MTZ_CU(h, cudaGetLastError());
 	if (sha) {
 		const unsigned gs = (unsigned)((nrec + SHA_THREADS - 1) / SHA_THREADS);
 		k_block_sha256<<<gs, SHA_THREADS, 0, st>>>(d_in, d_recs, d_out, orecs, (uint32_t)nrec, h->cfg.mode,
-		    base, bres);
+		    base, bres, fjobs);
 		MTZ_CU(h, cudaGetLastError());
 	}
 	if (sha512) {
 		const unsigned gs = (unsigned)((nrec + SHA512_THREADS - 1) / SHA512_THREADS);
 		k_block_sha512<<<gs, SHA512_THREADS, 0, st>>>(d_in, d_recs, d_out, orecs, (uint32_t)nrec, h->cfg.mode,
-		    base, bres);
+		    base, bres, fjobs);
 		MTZ_CU(h, cudaGetLastError());
 	}
 	return MTZ_OK;
+}
+
+static int32_t launch_k3(mtz_handle *h, cudaStream_t st, const void *d_src, void *d_dst,
+    mtz_job *d_jobs, uint32_t njobs, bool compact, const uint32_t *skip = nullptr, bool count = true);
+
+// The block check of a VERIFY (sub-)batch with MTZ_FLAG_BLOCK_FRAMES: plan, K3 and the frame sums into
+// cb's jobs / scratch / osums (kernels_frames.cuh), then launch_block against those frames.  The
+// headers of records [0, nrec) lie at d_in + rec.off with rec.off - base_off < cb.scratch_cap
+// (base_off 16-aligned); `compact` as for COMPRESS (all_compact_blocks).  Like the rest of the check,
+// nothing here is counted in mtz_stats.
+static int32_t launch_block_frames(mtz_handle *h, cudaStream_t st, CodecBufs &cb, const uint8_t *d_in,
+    const mtz_rec *d_recs, const RecSums *isums, size_t nrec, uint64_t base_off, bool compact, uint64_t base,
+    BlockResult *bres)
+{
+	if (nrec == 0) return MTZ_OK;
+	if (nrec > cb.rec_cap) return fail(h, MTZ_ENOSPC, "frame batch of %zu records exceeds %zu", nrec, cb.rec_cap);
+	const uint32_t n = (uint32_t)nrec;
+	k_frame_plan<<<(n + FRP_THREADS - 1) / FRP_THREADS, FRP_THREADS, 0, st>>>(d_in, d_recs, n, block_hashed(h),
+	    base_off, cb.d_enc, cb.enc);
+	MTZ_CU(h, cudaGetLastError());
+	int32_t rc = launch_k3(h, st, nullptr, nullptr, cb.enc, n, compact, nullptr, false);
+	if (rc != MTZ_OK) return rc;
+	const unsigned gs = (unsigned)std::min<size_t>((nrec + K1_WARPS - 1) / K1_WARPS, (size_t)h->sm_count * 16);
+	k_frame_sums<<<gs, K1_THREADS, 0, st>>>(cb.enc, n, cb.osums, bres);
+	MTZ_CU(h, cudaGetLastError());
+	return launch_block(h, st, d_in, d_recs, isums, nullptr, cb.osums, nullptr, nrec, base, bres, cb.enc);
 }
 
 // Merge a batch's results (host copy) into `p`; on a mismatch read drr_object / drr_offset of the
@@ -598,7 +639,7 @@ static int32_t block_take(mtz_handle *h, BlockPending &p, const BlockResult &r, 
 {
 	p.r.logical_ok += r.logical_ok; p.r.frame_ok += r.frame_ok;
 	p.r.frame_miss += r.frame_miss; p.r.skipped += r.skipped; p.r.sha256 += r.sha256;
-	p.r.sha512 += r.sha512;
+	p.r.sha512 += r.sha512; p.r.frames += r.frames;
 	p.r.first_miss = std::min(p.r.first_miss, r.first_miss);
 	if (r.first_bad < p.r.first_bad) {
 		uint64_t w[6];      // header bytes 8..55: drr_object, drr_offset, drr_checksumtype
@@ -621,6 +662,7 @@ static int32_t block_fold(mtz_handle *h, BlockPending &p, uint64_t stream_bad)
 		h->bstats.logical_ok += q.r.logical_ok; h->bstats.frame_ok += q.r.frame_ok;
 		h->bstats.frame_miss += q.r.frame_miss; h->bstats.skipped += q.r.skipped;
 		h->bstats.sha256 += q.r.sha256; h->bstats.sha512 += q.r.sha512;
+		h->bstats.frames_encoded += q.r.frames;
 		h->bstats.first_frame_miss = std::min<uint64_t>(h->bstats.first_frame_miss, q.r.first_miss);
 	}
 	if (q.r.first_bad == ~0ull || q.r.first_bad >= stream_bad) return MTZ_OK;
@@ -682,7 +724,8 @@ static int32_t codec_alloc(mtz_handle *h, CodecBufs &cb, size_t rec_cap, size_t 
 	MTZ_CU(h, cudaMalloc(&cb.out_recs, rec_cap * sizeof(mtz_rec)));
 	MTZ_CU(h, cudaMalloc(&cb.osums, rec_cap * sizeof(RecSums)));
 	MTZ_CU(h, cudaMalloc(&cb.steps, rec_cap * sizeof(StampStep)));
-	if (h->cfg.mode != MTZ_MODE_COMPRESS) MTZ_CU(h, cudaMalloc(&cb.d_logical, scratch_cap + 512));
+	if (h->cfg.mode == MTZ_MODE_DECOMPRESS || h->cfg.mode == MTZ_MODE_RECOMPRESS)
+		MTZ_CU(h, cudaMalloc(&cb.d_logical, scratch_cap + 512));
 	if (h->cfg.mode != MTZ_MODE_DECOMPRESS) MTZ_CU(h, cudaMalloc(&cb.d_enc, scratch_cap + 512));
 	if (certify_on(h)) {
 		MTZ_CU(h, cudaMalloc(&cb.seq_n, rec_cap * sizeof(uint32_t)));
@@ -720,8 +763,6 @@ static int32_t codec_reset(mtz_handle *h, cudaStream_t st, CodecBufs &cb)
 
 // Part 1 of the re-encoding pipeline of one (sub-)batch: plan + K2 + K3.  It
 // does not touch the running checksums, so it may run ahead of the chain.
-static int32_t launch_k3(mtz_handle *h, cudaStream_t st, const void *d_src, void *d_dst,
-    mtz_job *d_jobs, uint32_t njobs, bool compact, const uint32_t *skip = nullptr);
 static int32_t launch_k3c(mtz_handle *h, cudaStream_t st, CodecBufs &cb, uint32_t njobs, bool compact);
 
 // true when every DRR_WRITE of the table has a 128 KiB-class logical size
@@ -861,6 +902,75 @@ int32_t mtz_set_carry(mtz_handle *h, const uint64_t carry_in[4], const uint64_t 
 	return MTZ_OK;
 }
 
+// The device API's scratch.  dv_cb: the codec sub-batches, or in VERIFY the frames of the block check
+// (MTZ_FLAG_BLOCK_FRAMES); the codec modes also get a second set and the streams and events of their
+// three-stream pipeline.
+static int32_t dv_alloc(mtz_handle *h)
+{
+	if (h->dv_cb.cr != nullptr) return MTZ_OK;
+	const size_t scratch = std::max<size_t>(2ull << 30, (size_t)h->cfg.batch_bytes + MAX_RECORD_BYTES);
+	int32_t rc = codec_alloc(h, h->dv_cb, 65536, scratch);
+	if (rc != MTZ_OK || !is_codec_mode(h->cfg.mode)) return rc;
+	rc = codec_alloc(h, h->dv_cb2, 65536, scratch);
+	if (rc != MTZ_OK) return rc;
+	// one set of results / running output offset for the whole submit
+	cudaFree(h->dv_cb2.d_cres); cudaFree(h->dv_cb2.d_ores); cudaFree(h->dv_cb2.d_outpos);
+	cudaFreeHost(h->dv_cb2.h_cres); cudaFreeHost(h->dv_cb2.h_ores);
+	h->dv_cb2.d_cres = h->dv_cb.d_cres; h->dv_cb2.d_ores = h->dv_cb.d_ores;
+	h->dv_cb2.d_outpos = h->dv_cb.d_outpos;
+	h->dv_cb2.h_cres = h->dv_cb.h_cres; h->dv_cb2.h_ores = h->dv_cb.h_ores;
+	MTZ_CU(h, cudaEventCreate(&h->dv_c0));
+	MTZ_CU(h, cudaEventCreate(&h->dv_c1));
+	MTZ_CU(h, make_stream(&h->st_post, true));
+	MTZ_CU(h, make_stream(&h->st_dec, true));
+	for (int i = 0; i < 2; i++) {
+		MTZ_CU(h, cudaEventCreateWithFlags(&h->ev_dec[i], cudaEventDisableTiming));
+		MTZ_CU(h, cudaEventCreateWithFlags(&h->ev_pre[i], cudaEventDisableTiming));
+		if (i == 0) MTZ_CU(h, cudaEventCreateWithFlags(&h->ev_reset, cudaEventDisableTiming));
+		MTZ_CU(h, cudaEventCreateWithFlags(&h->ev_post[i], cudaEventDisableTiming));
+	}
+	return MTZ_OK;
+}
+
+// host copy of the submit's record table (dv_hrecs): the sub-batches are cut on the host
+static int32_t dv_host_recs(mtz_handle *h, cudaStream_t st, const mtz_rec *d_recs, size_t nrec)
+{
+	h->dv_hrecs.resize(nrec);
+	MTZ_CU(h, cudaMemcpyAsync(h->dv_hrecs.data(), d_recs, nrec * sizeof(mtz_rec), cudaMemcpyDeviceToHost, st));
+	MTZ_CU(h, cudaStreamSynchronize(st));
+	return MTZ_OK;
+}
+
+// The block check of a VERIFY submit with MTZ_FLAG_BLOCK_FRAMES, in sub-batches whose input span fits
+// dv_cb's scratch (2 GiB) and whose records fit its tables; one after another on `st`, verdicts into
+// dv_bres for the finish.
+static int32_t dv_block_frames(mtz_handle *h, cudaStream_t st, const uint8_t *d_in, const mtz_rec *d_recs,
+    size_t nrec)
+{
+	int32_t rc = dv_alloc(h);
+	if (rc == MTZ_OK) rc = dv_host_recs(h, st, d_recs, nrec);
+	if (rc != MTZ_OK) return rc;
+	const CodecBufs &cb = h->dv_cb;
+	const mtz_rec *hr = h->dv_hrecs.data();
+	for (size_t i0 = 0; i0 < nrec;) {
+		const uint64_t base_off = hr[i0].off & ~15ull;
+		size_t i1 = i0;
+		while (i1 < nrec && i1 - i0 < cb.rec_cap) {
+			const uint64_t end = hr[i1].off + DRR_HDR + hr[i1].payload;
+			if (end - base_off > cb.scratch_cap) {
+				if (i1 == i0) return fail(h, MTZ_ENOSPC, "record exceeds the frame scratch");
+				break;
+			}
+			i1++;
+		}
+		rc = launch_block_frames(h, st, h->dv_cb, d_in, d_recs + i0, h->dv_sums + i0, i1 - i0, base_off,
+		    all_compact_blocks(hr + i0, i1 - i0), h->dv_first + i0, h->dv_bres);
+		if (rc != MTZ_OK) return rc;
+		i0 = i1;
+	}
+	return MTZ_OK;
+}
+
 int32_t mtz_dev_submit(mtz_handle *h, const void *d_in, size_t in_bytes,
     const mtz_rec *d_recs, size_t nrec, void *d_out, size_t out_cap, void *cuda_stream)
 {
@@ -884,7 +994,9 @@ int32_t mtz_dev_submit(mtz_handle *h, const void *d_in, size_t in_bytes,
 	if (h->dv_bres_live) {
 		h->dv_in = (const uint8_t *)d_in; h->dv_recs = d_recs;
 		rc = block_reset(h, st, h->dv_bres);
-		if (rc == MTZ_OK && !is_codec_mode(h->cfg.mode))
+		if (rc == MTZ_OK && block_frames_on(h))
+			rc = dv_block_frames(h, st, (const uint8_t *)d_in, d_recs, nrec);
+		else if (rc == MTZ_OK && !is_codec_mode(h->cfg.mode))
 			rc = launch_block(h, st, (const uint8_t *)d_in, d_recs, h->dv_sums, nullptr, nullptr, nullptr,
 			    nrec, h->dv_first, h->dv_bres);
 		if (rc != MTZ_OK) return rc;
@@ -896,32 +1008,10 @@ int32_t mtz_dev_submit(mtz_handle *h, const void *d_in, size_t in_bytes,
 	// overlap layout/assemble/sums/stamp-chain of sub-batch k (stream st_post); the
 	// chain is one warp on one SM and would otherwise serialise ~12 % of the step.
 	if (d_out == nullptr) return fail(h, MTZ_EINVAL, "codec modes need d_out");
-	if (h->dv_cb.cr == nullptr) {
-		const size_t scratch = std::max<size_t>(2ull << 30, (size_t)h->cfg.batch_bytes + MAX_RECORD_BYTES);
-		rc = codec_alloc(h, h->dv_cb, 65536, scratch);
-		if (rc != MTZ_OK) return rc;
-		rc = codec_alloc(h, h->dv_cb2, 65536, scratch);
-		if (rc != MTZ_OK) return rc;
-		// one set of results / running output offset for the whole submit
-		cudaFree(h->dv_cb2.d_cres); cudaFree(h->dv_cb2.d_ores); cudaFree(h->dv_cb2.d_outpos);
-		cudaFreeHost(h->dv_cb2.h_cres); cudaFreeHost(h->dv_cb2.h_ores);
-		h->dv_cb2.d_cres = h->dv_cb.d_cres; h->dv_cb2.d_ores = h->dv_cb.d_ores;
-		h->dv_cb2.d_outpos = h->dv_cb.d_outpos;
-		h->dv_cb2.h_cres = h->dv_cb.h_cres; h->dv_cb2.h_ores = h->dv_cb.h_ores;
-		MTZ_CU(h, cudaEventCreate(&h->dv_c0));
-		MTZ_CU(h, cudaEventCreate(&h->dv_c1));
-		MTZ_CU(h, make_stream(&h->st_post, true));
-		MTZ_CU(h, make_stream(&h->st_dec, true));
-		for (int i = 0; i < 2; i++) {
-			MTZ_CU(h, cudaEventCreateWithFlags(&h->ev_dec[i], cudaEventDisableTiming));
-			MTZ_CU(h, cudaEventCreateWithFlags(&h->ev_pre[i], cudaEventDisableTiming));
-			if (i == 0) MTZ_CU(h, cudaEventCreateWithFlags(&h->ev_reset, cudaEventDisableTiming));
-			MTZ_CU(h, cudaEventCreateWithFlags(&h->ev_post[i], cudaEventDisableTiming));
-		}
-	}
-	h->dv_hrecs.resize(nrec);
-	MTZ_CU(h, cudaMemcpyAsync(h->dv_hrecs.data(), d_recs, nrec * sizeof(mtz_rec), cudaMemcpyDeviceToHost, st));
-	MTZ_CU(h, cudaStreamSynchronize(st));
+	rc = dv_alloc(h);
+	if (rc != MTZ_OK) return rc;
+	rc = dv_host_recs(h, st, d_recs, nrec);
+	if (rc != MTZ_OK) return rc;
 	rc = codec_reset(h, st, h->dv_cb);
 	if (rc != MTZ_OK) return rc;
 	size_t need_out = 0;
@@ -1291,6 +1381,8 @@ static int32_t ensure_slots(mtz_handle *h)
 		if (is_codec_mode(h->cfg.mode)) {
 			s.out_cap = cap;
 			MTZ_CU(h, cudaMalloc(&s.d_out, cap + 512));
+		}
+		if (is_codec_mode(h->cfg.mode) || block_frames_on(h)) {
 			rc = codec_alloc(h, s.cb, rec_cap, cap + rec_cap * 48);
 			if (rc != MTZ_OK) return rc;
 		}
@@ -1463,7 +1555,10 @@ static int32_t submit_batch(mtz_handle *h, Slot &s, const uint8_t *p0, size_t n0
 		// the block check needs no running checksum: it runs now, its verdict waits with the stream's
 		if (block_on(h) && nrec > 0) {
 			rc = block_reset(h, s.st, s.d_bres);
-			if (rc == MTZ_OK)
+			if (rc == MTZ_OK && block_frames_on(h))
+				rc = launch_block_frames(h, s.st, s.cb, s.d_in, s.d_recs, h->dv_sums + h->dv_nrec, nrec, 0,
+				    all_compact_blocks(s.h_recs, nrec), s.first_rec, s.d_bres);
+			else if (rc == MTZ_OK)
 				rc = launch_block(h, s.st, s.d_in, s.d_recs, h->dv_sums + h->dv_nrec, nullptr, nullptr, nullptr,
 				    nrec, s.first_rec, s.d_bres);
 			if (rc != MTZ_OK) return rc;
@@ -1478,7 +1573,10 @@ static int32_t submit_batch(mtz_handle *h, Slot &s, const uint8_t *p0, size_t n0
 		if (block_on(h) && nrec > 0) {
 			// VERIFY checks the input here; the codec modes after the output's sums (codec_launch_post)
 			rc = block_reset(h, s.st, s.d_bres);
-			if (rc == MTZ_OK && !is_codec_mode(h->cfg.mode))
+			if (rc == MTZ_OK && block_frames_on(h))
+				rc = launch_block_frames(h, s.st, s.cb, s.d_in, s.d_recs, s.d_sums, nrec, 0,
+				    all_compact_blocks(s.h_recs, nrec), s.first_rec, s.d_bres);
+			else if (rc == MTZ_OK && !is_codec_mode(h->cfg.mode))
 				rc = launch_block(h, s.st, s.d_in, s.d_recs, s.d_sums, nullptr, nullptr, nullptr, nrec, s.first_rec,
 				    s.d_bres);
 			if (rc != MTZ_OK) return rc;
@@ -1738,9 +1836,10 @@ static int32_t k3_set_attributes(mtz_handle *h)
 	return MTZ_OK;
 }
 
-// compact = every block is 64 KiB+11 .. 128 KiB: 8.5 KiB tables, more warps per SM
+// compact = every block is 64 KiB+11 .. 128 KiB: 8.5 KiB tables, more warps per SM.  `count` = the
+// launch is counted in mtz_stats.kernel_launches (not the block check's, launch_block_frames)
 static int32_t launch_k3(mtz_handle *h, cudaStream_t st, const void *d_src, void *d_dst,
-    mtz_job *d_jobs, uint32_t njobs, bool compact, const uint32_t *skip)
+    mtz_job *d_jobs, uint32_t njobs, bool compact, const uint32_t *skip, bool count)
 {
 	const size_t tabw = compact ? LZ4_TAB_COMPACT_WORDS : LZ4_TAB_BIG_WORDS;
 	const size_t smem = (size_t)K3_WARPS * tabw * sizeof(uint32_t);
@@ -1757,7 +1856,7 @@ static int32_t launch_k3(mtz_handle *h, cudaStream_t st, const void *d_src, void
 	else
 		k3_lz4_encode<false><<<grid, K3_THREADS, smem, st>>>((const uint8_t *)d_src, (uint8_t *)d_dst, d_jobs, njobs, skip);
 	MTZ_CU(h, cudaGetLastError());
-	count_launch(h, 1);
+	if (count) count_launch(h, 1);
 	return MTZ_OK;
 }
 

@@ -133,7 +133,8 @@ class BackupSender(object):
                                 out_ring_bytes=g.get("outRingBytes", 0), n_slots=g.get("slots", 0),
                                 block_checksums=bool(g.get("blockChecksums")),
                                 block_sha256=bool(g.get("blockSha256")),
-                                block_sha512=bool(g.get("blockSha512")))
+                                block_sha512=bool(g.get("blockSha512")),
+                                block_frames=bool(g.get("blockFrames")))
 
     def _stage_stats(self, stage):
         """job.gpu: the stage counters, plus `blocks` (block-checksum counters) with

@@ -122,7 +122,8 @@ class ZfsClient(object):
                                 out_ring_bytes=g.get("outRingBytes", 0), n_slots=g.get("slots", 0),
                                 block_checksums=bool(g.get("blockChecksums")),
                                 block_sha256=bool(g.get("blockSha256")),
-                                block_sha512=bool(g.get("blockSha512")))
+                                block_sha512=bool(g.get("blockSha512")),
+                                block_frames=bool(g.get("blockFrames")))
 
     def _wire_mode(self, serverUrl, jobPath):
         """Which stage to put in the pipe for THIS job (SURVEY.md 8f f2).  A receiver configured

@@ -37,6 +37,8 @@ PARAMS = {
     "test_lz4_on_disk_sha512_keys": [(9,), (12,)],
     "test_one_stream_mixing_fletcher4_sha256_sha512_and_skipped_keys": [(False, False), (True, False),
                                                                         (False, True), (True, True)],
+    "test_lz4_on_disk_keys_match_the_encoder_in_verify": [(9, 512), (9, 8192), (12, 8192), (12, 131072)],
+    "test_sha256_and_sha512_lz4_on_disk_keys": [(9,), (12,)],
 }
 SKIP = {"test_sixteen_mib_record": "16 MiB blocks take minutes per encode on the emulator",
         "test_size_independent_properties_at_2gib": "2 GiB of LZ4 work is out of reach for the emulator",
@@ -58,12 +60,13 @@ def main():
     import test_gpu_block_cksum as B
     import test_gpu_block_sha256 as H
     import test_gpu_block_sha512 as W
+    import test_gpu_block_frames as F
     import test_gpu_codec as K
     import test_gpu_lz4 as Z
     import test_gpu_stream as S
     import test_gpu_verify as V
     tot = fail = 0
-    for mod in (V, S, Z, K, B, H, W):
+    for mod in (V, S, Z, K, B, H, W, F):
         for name, fn in inspect.getmembers(mod, inspect.isfunction):
             if not name.startswith("test_") or filt not in name:
                 continue
