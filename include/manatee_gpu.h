@@ -90,6 +90,17 @@ extern "C" {
                                   * frames; with this flag and batch_bytes 0 VERIFY batches are 256 MiB.
                                   * The other modes accept the flag and do not change */
 
+#define MTZ_FLAG_BLOCK_LZJB 64u  /* with MTZ_FLAG_BLOCK_CKSUM only (MTZ_EINVAL without it), with or without
+                                  * BLOCK_FRAMES and the SHA flags.  Keys over an lzjb (on-disk compression 3)
+                                  * or zle (14) frame are checked, otherwise skipped.  VERIFY and RECOMPRESS:
+                                  * a record that arrives as that frame (send -c) is compared as it is.
+                                  * VERIFY: a record that arrives raw gets a frame from the stage's lzjb / zle
+                                  * encoder (ZFS's, at buffer address phase 0).  Either way the verdict is
+                                  * frame_ok or frame_miss (counted, never an error) and the output bytes do
+                                  * not change.  mtz_block_stats.lzjb_encoded / zle_encoded count the frames
+                                  * encoded; with this flag and batch_bytes 0 VERIFY batches are 256 MiB.
+                                  * COMPRESS and DECOMPRESS accept the flag and do not change */
+
 typedef struct mtz_handle mtz_handle;
 
 #define MTZ_MAX_DEVICES 16
@@ -103,7 +114,7 @@ typedef struct mtz_config {
 	uint64_t ring_bytes;    /* pinned input ring (0 = max(256 MiB, 2 x batch_bytes)) */
 	uint64_t out_ring_bytes;/* pinned output ring, codec modes (0 = ring_bytes) */
 	uint64_t batch_bytes;   /* target bytes per GPU batch (0 = 32 MiB; 256 MiB in codec modes and
-	                         * with MTZ_FLAG_BLOCK_FRAMES) */
+	                         * with MTZ_FLAG_BLOCK_FRAMES or MTZ_FLAG_BLOCK_LZJB) */
 	uint32_t record_bytes;  /* expected recordsize hint (0 = 131072) */
 	uint32_t n_slots;       /* batches in flight PER DEVICE (0 = 4) */
 	/* ---- ABI v2: the GPUs of one box as ONE stage.  The stream is cut into whole-record
@@ -145,7 +156,7 @@ typedef struct mtz_block_stats {
 	uint32_t struct_size;       /* sizeof(mtz_block_stats), set by the caller */
 	uint32_t pad;
 	uint64_t logical_ok;        /* stored raw on disk: logical bytes match the key */
-	uint64_t frame_ok;          /* stored LZ4 on disk: the frame at hand matches the key */
+	uint64_t frame_ok;          /* stored compressed on disk: the frame at hand matches the key */
 	uint64_t frame_miss;        /* ... does not: another encoder wrote the disk block */
 	uint64_t skipped;
 	uint64_t first_frame_miss;  /* stream index of the first frame miss, ~0 if none */
@@ -154,6 +165,8 @@ typedef struct mtz_block_stats {
 	uint64_t sha512;            /* MTZ_FLAG_BLOCK_SHA512: records compared by SHA-512/256 (likewise) */
 	uint64_t frames_encoded;    /* MTZ_FLAG_BLOCK_FRAMES: frames encoded for the check (also counted in
 	                               frame_ok / frame_miss, and in sha256 / sha512 where those hashed it) */
+	uint64_t lzjb_encoded;      /* MTZ_FLAG_BLOCK_LZJB: lzjb frames encoded for the check (likewise) */
+	uint64_t zle_encoded;       /* MTZ_FLAG_BLOCK_LZJB: zle frames encoded for the check (likewise) */
 } mtz_block_stats;
 
 /* One DRR record as seen by the kernels (32 B, little endian). */

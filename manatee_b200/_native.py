@@ -21,6 +21,7 @@ FLAG_BLOCK_CKSUM = 4
 FLAG_BLOCK_SHA256 = 8
 FLAG_BLOCK_SHA512 = 16
 FLAG_BLOCK_FRAMES = 32
+FLAG_BLOCK_LZJB = 64
 XCHG_FIRST, XCHG_LAST = 1, 2
 MODE_NAMES = {"verify": 0, "compress": 1, "decompress": 2, "recompress": 3, "passthrough": 4}
 
@@ -55,7 +56,8 @@ class BlockStats(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("pad", C.c_uint32), ("logical_ok", C.c_uint64),
                 ("frame_ok", C.c_uint64), ("frame_miss", C.c_uint64), ("skipped", C.c_uint64),
                 ("first_frame_miss", C.c_uint64), ("sha256", C.c_uint64),
-                ("sha512", C.c_uint64), ("frames_encoded", C.c_uint64)]
+                ("sha512", C.c_uint64), ("frames_encoded", C.c_uint64),
+                ("lzjb_encoded", C.c_uint64), ("zle_encoded", C.c_uint64)]
 
     def as_dict(self):
         return {k: getattr(self, k) for k, _ in self._fields_[2:]}

@@ -22,12 +22,19 @@ namespace mtz {
 #define BLK_DC_INHERIT 0u      // "stored raw": the key covers the logical block
 #define BLK_DC_OFF     2u
 #define BLK_DC_LZ4     15u     // the key covers ZFS's LZ4 frame, zero-padded to PSIZE
+#define BLK_DC_LZJB    3u      // ... its lzjb frame (kernels_lzjb.cuh)
+#define BLK_DC_ZLE     14u     // ... its zle frame (kernels_lzjb.cuh)
+// block_classify's `frames`: the frames VERIFY encodes for the check (kernels_frames.cuh)
+#define BLK_FR_LZ4     1u      // MTZ_FLAG_BLOCK_FRAMES: LZ4 frames (K3)
+#define BLK_FR_LZJB    2u      // MTZ_FLAG_BLOCK_LZJB: lzjb and zle frames, and in VERIFY and
+                               // RECOMPRESS lzjb / zle records that arrive as their disk frame
 
 struct BlockResult {           // device, mirrored to pinned host; zeroed per batch
 	unsigned long long logical_ok, frame_ok, frame_miss, skipped;
 	unsigned long long sha256;       // records compared by k_block_sha256 (kernels_sha256.cuh)
 	unsigned long long sha512;       // records compared by k_block_sha512 (kernels_sha512.cuh)
-	unsigned long long frames;       // frames encoded for the check (k_frame_sums, kernels_frames.cuh)
+	unsigned long long frames;       // LZ4 frames encoded for the check (k_frame_sums, kernels_frames.cuh)
+	unsigned long long lzjb, zle;    // lzjb / zle frames encoded for the check (likewise)
 	unsigned long long first_bad;    // stream index of the first logical mismatch, ~0 none
 	unsigned long long first_miss;   // stream index of the first frame mismatch, ~0 none
 };
@@ -48,16 +55,18 @@ __host__ __device__ __forceinline__ Ck4 strip_head8(const Ck4 &whole, const Ck4 
 // What a record's key lets the stage compare, decided from its header alone, for keys of type
 // `ctype`: `what` 0 skipped, 1 the logical block, 2 the disk frame; `src` 0 the input payload, 1 the
 // output payload, or in VERIFY the frame the declared encoder made of the input (kernels_frames.cuh).
-// `have_out` = the output records of a re-encoding mode are at hand; `frames` = VERIFY with
-// MTZ_FLAG_BLOCK_FRAMES: the encoder's frames of the raw records are.  Every key type that is
-// checked goes through this one table.
+// `have_out` = the output records of a re-encoding mode are at hand; `frames` = BLK_FR_* bits: with
+// BLK_FR_LZ4 (VERIFY with MTZ_FLAG_BLOCK_FRAMES) the encoder's LZ4 frames of the raw records are, with
+// BLK_FR_LZJB (MTZ_FLAG_BLOCK_LZJB) lzjb and zle keys are checked: against the input payload when
+// the record arrives as that frame (VERIFY, RECOMPRESS: passed through), in VERIFY against the
+// encoder's frame of a raw record.  Every key type that is checked goes through this one table.
 struct BlockClass {
 	int what, src;
 	uint64_t lsz, psz;
 };
 
 __device__ __forceinline__ BlockClass block_classify(const uint8_t *hdr, const mtz_rec &rec, uint32_t mode,
-    bool have_out, uint32_t ctype, bool frames = false)
+    bool have_out, uint32_t ctype, uint32_t frames = 0u)
 {
 	const uint64_t prop = *reinterpret_cast<const uint64_t *>(hdr + 88);
 	BlockClass c;
@@ -73,7 +82,10 @@ __device__ __forceinline__ BlockClass block_classify(const uint8_t *hdr, const m
 			else if (lz4_in && mode == MTZ_MODE_DECOMPRESS && have_out) { c.what = 1; c.src = 1; }
 		} else if (dc == BLK_DC_LZ4) {
 			if (lz4_in) { c.what = 2; c.src = 0; }
-			else if (raw_in && ((encodes && have_out) || (frames && mode == MTZ_MODE_VERIFY))) { c.what = 2; c.src = 1; }
+			else if (raw_in && ((encodes && have_out) || ((frames & BLK_FR_LZ4) && mode == MTZ_MODE_VERIFY))) { c.what = 2; c.src = 1; }
+		} else if ((frames & BLK_FR_LZJB) && (dc == BLK_DC_LZJB || dc == BLK_DC_ZLE)) {
+			if (rec.comp == dc && (mode == MTZ_MODE_VERIFY || mode == MTZ_MODE_RECOMPRESS)) { c.what = 2; c.src = 0; }
+			else if (raw_in && mode == MTZ_MODE_VERIFY) { c.what = 2; c.src = 1; }
 		}
 	}
 	return c;
@@ -98,22 +110,22 @@ __device__ __forceinline__ void block_verdict(BlockResult *res, int what, bool o
 // is record `base + r` of the stream.  `hashed` has bit t set for each key type t another kernel
 // hashes (bit 8: k_block_sha256 with MTZ_FLAG_BLOCK_SHA256, bit 11: k_block_sha512 with
 // MTZ_FLAG_BLOCK_SHA512): the keys of those types this stage can check are left to that kernel
-// instead of being counted as skipped.  `fjobs` (VERIFY with MTZ_FLAG_BLOCK_FRAMES, else null): the
-// K3 jobs of kernels_frames.cuh, whose frames stand in for the output records and whose sums are in
-// `osums`.
+// instead of being counted as skipped.  `fjobs` (VERIFY with MTZ_FLAG_BLOCK_FRAMES or
+// MTZ_FLAG_BLOCK_LZJB, else null): the frame jobs of kernels_frames.cuh, whose frames stand in for the
+// output records and whose sums are in `osums`.  `frames`: block_classify's BLK_FR_* bits.
 #define BLK_THREADS 128
 __global__ void __launch_bounds__(BLK_THREADS)
 k_block_check(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs,
     const RecSums *__restrict__ isums, const mtz_rec *__restrict__ orecs,
     const RecSums *__restrict__ osums, uint32_t n, uint32_t mode, uint64_t base,
-    BlockResult *__restrict__ res, uint32_t hashed, const mtz_job *__restrict__ fjobs = nullptr)
+    BlockResult *__restrict__ res, uint32_t hashed, const mtz_job *__restrict__ fjobs = nullptr,
+    uint32_t frames = 0u)
 {
 	const uint32_t r = blockIdx.x * BLK_THREADS + threadIdx.x;
 	if (r >= n) return;
 	const mtz_rec rec = recs[r];
 	if (rec.type != DRR_WRITE_T) return;
 	const uint8_t *hdr = d_in + rec.off;
-	const bool frames = fjobs != nullptr;
 	const BlockClass c = block_classify(hdr, rec, mode, osums != nullptr, ZIO_CKSUM_FLETCHER4, frames);
 	const int what = c.what, src = c.src;
 	if (what == 0) {
@@ -130,7 +142,7 @@ k_block_check(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs
 		const Ck4 zero = { 0, 0, 0, 0 };
 		nbytes = (uint64_t)rec.payload;
 		sums = strip_head8(s.body, fold_cksum_words(zero, s.emb), s.nbody - 8u);
-	} else if (!frames) {
+	} else if (fjobs == nullptr) {
 		const mtz_rec o = orecs[r];
 		nbytes = (uint64_t)o.payload;
 		sums = osums[r].body;

@@ -1,27 +1,33 @@
-// kernels_frames.cuh -- the frames of the block check in VERIFY (MTZ_FLAG_BLOCK_FRAMES).  A block
-// ZFS stored LZ4 has a key over its disk frame, zero-padded to PSIZE; a VERIFY stage that receives
-// the block raw (`zfs send` without -c) has no frame to compare.  With the flag it makes one with
-// the declared encoder (K3, unchanged) into a scratch beside the batch, and the checks compare that
-// frame by the rules of COMPRESS, which compares its own encoder output: the stage hands on the
-// input bytes untouched either way.
-//   k_frame_plan  one K3 job per record: the raw records whose key covers an LZ4 frame (the
-//                 decision is block_classify's), an empty job for every other record
-//   K3            k3_lz4_encode over those jobs: out_len = PSIZE of the frame, or lsize = stored raw
+// kernels_frames.cuh -- the frames of the block check in VERIFY (MTZ_FLAG_BLOCK_FRAMES,
+// MTZ_FLAG_BLOCK_LZJB).  A block ZFS stored compressed has a key over its disk frame, zero-padded to
+// PSIZE; a VERIFY stage that receives the block raw (`zfs send` without -c) has no frame to compare.
+// With the flags it makes one with the declared encoder into a scratch beside the batch, and the
+// checks compare that frame by the rules of COMPRESS, which compares its own encoder output: the
+// stage hands on the input bytes untouched either way.
+//   k_frame_plan  one job per record: the raw records whose key covers an LZ4 (MTZ_FLAG_BLOCK_FRAMES),
+//                 lzjb or zle frame (MTZ_FLAG_BLOCK_LZJB), the decision block_classify's and the codec
+//                 in the job's src_len; an empty job for every other record
+//   K3            k3_lz4_encode over the LZ4 jobs: out_len = PSIZE of the frame, or lsize = stored raw
+//   k_lzjb_encode, k_zle_encode (kernels_lzjb.cuh): likewise over the lzjb and zle jobs
 //   k_frame_sums  Fletcher-4 sums of each frame, one warp per record (warp_fletcher rows)
 // k_block_check, k_block_sha256 and k_block_sha512 then read the frame through the jobs.
 #pragma once
 #include "kernels_block.cuh"
+#include "kernels_lzjb.cuh"
 
 namespace mtz {
 
 // Record r's slot is scratch + (rec.off & ~15) - base_off: its frame is at most lsize bytes and the
 // record itself spans 312 + lsize bytes of the batch, so the slots of a batch do not overlap and
 // the scratch needs no more bytes than the batch (base_off 16-aligned, at or before the first
-// header).  `hashed` as k_block_check's: the key types checked besides fletcher4.
+// header).  `hashed` as k_block_check's: the key types checked besides fletcher4; `frames`:
+// block_classify's BLK_FR_* bits.  A job's src_len is its codec (BLK_DC_LZ4 / _LZJB / _ZLE).
+// `k3_skip` (null unless both flags are on): 1 for each job K3 must leave to the other encoders.
 #define FRP_THREADS 128
 __global__ void __launch_bounds__(FRP_THREADS)
 k_frame_plan(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs, uint32_t n,
-    uint32_t hashed, uint64_t base_off, uint8_t *scratch, mtz_job *__restrict__ jobs)
+    uint32_t hashed, uint64_t base_off, uint8_t *scratch, mtz_job *__restrict__ jobs, uint32_t frames,
+    uint32_t *__restrict__ k3_skip)
 {
 	const uint32_t r = blockIdx.x * FRP_THREADS + threadIdx.x;
 	if (r >= n) return;
@@ -32,8 +38,9 @@ k_frame_plan(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs,
 		const uint8_t *hdr = d_in + rec.off;
 		const uint32_t t = hdr[48];
 		if (t == ZIO_CKSUM_FLETCHER4 || (t < 32u && ((hashed >> t) & 1u))) {
-			const BlockClass c = block_classify(hdr, rec, MTZ_MODE_VERIFY, false, t, true);
+			const BlockClass c = block_classify(hdr, rec, MTZ_MODE_VERIFY, false, t, frames);
 			if (c.what == 2 && c.src == 1) {
+				j.src_len = (uint32_t)((*reinterpret_cast<const uint64_t *>(hdr + 88) >> 32) & 0x7full);
 				j.src_off = (uint64_t)(uintptr_t)(hdr + DRR_HDR);
 				j.dst_off = (uint64_t)(uintptr_t)(scratch + ((rec.off & ~15ull) - base_off));
 				j.lsize = rec.lsize;
@@ -41,10 +48,11 @@ k_frame_plan(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs,
 		}
 	}
 	jobs[r] = j;
+	if (k3_skip != nullptr) k3_skip[r] = j.src_len != BLK_DC_LZ4;
 }
 
-// One warp per record (grid-stride): zero-state sums of the frame K3 left at jobs[r].dst_off into
-// sums[r].body, and the record counted in res->frames.  A frame the encoder stored raw (out_len ==
+// One warp per record (grid-stride): zero-state sums of the frame its encoder left at jobs[r].dst_off
+// into sums[r].body, and the record counted in res->frames, res->lzjb or res->zle by its codec.  A frame the encoder stored raw (out_len ==
 // lsize) has no sums: the checks count it as a miss without reading them.
 __global__ void __launch_bounds__(K1_THREADS)
 k_frame_sums(const mtz_job *__restrict__ jobs, uint32_t n, RecSums *__restrict__ sums,
@@ -71,7 +79,7 @@ k_frame_sums(const mtz_job *__restrict__ jobs, uint32_t n, RecSums *__restrict__
 		}
 		if (lane == 0) {
 			sums[r].body = acc;
-			atomicAdd(&res->frames, 1ull);
+			atomicAdd(j.src_len == BLK_DC_LZJB ? &res->lzjb : j.src_len == BLK_DC_ZLE ? &res->zle : &res->frames, 1ull);
 		}
 	}
 }

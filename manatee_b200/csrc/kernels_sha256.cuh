@@ -107,14 +107,15 @@ __device__ __forceinline__ void sha256_message_block(const uint8_t *__restrict__
 __global__ void __launch_bounds__(SHA_THREADS)
 k_block_sha256(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs,
     const uint8_t *__restrict__ d_out, const mtz_rec *__restrict__ orecs, uint32_t n, uint32_t mode,
-    uint64_t base, BlockResult *__restrict__ res, const mtz_job *__restrict__ fjobs = nullptr)
+    uint64_t base, BlockResult *__restrict__ res, const mtz_job *__restrict__ fjobs = nullptr,
+    uint32_t frames = 0u)
 {
 	const uint32_t r = blockIdx.x * SHA_THREADS + threadIdx.x;
 	if (r >= n) return;
 	const mtz_rec rec = recs[r];
 	if (rec.type != DRR_WRITE_T) return;
 	const uint8_t *hdr = d_in + rec.off;
-	const BlockClass c = block_classify(hdr, rec, mode, orecs != nullptr, ZIO_CKSUM_SHA256, fjobs != nullptr);
+	const BlockClass c = block_classify(hdr, rec, mode, orecs != nullptr, ZIO_CKSUM_SHA256, frames);
 	if (c.what == 0) return;
 	const uint8_t *p;
 	uint64_t nbytes;
@@ -129,7 +130,7 @@ k_block_sha256(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ rec
 		// the stage's encoder stored the block raw where ZFS's stored a frame: not that encoder
 		if (c.what == 2 && o.comp != ZIO_LZ4) ok = false;
 	} else {
-		// VERIFY with MTZ_FLAG_BLOCK_FRAMES: the declared encoder's frame (kernels_frames.cuh)
+		// VERIFY with MTZ_FLAG_BLOCK_FRAMES / _LZJB: the declared encoder's frame (kernels_frames.cuh)
 		const mtz_job j = fjobs[r];
 		p = reinterpret_cast<const uint8_t *>((uintptr_t)j.dst_off);
 		nbytes = (uint64_t)j.out_len;

@@ -30,7 +30,7 @@ struct BlockPending {
 	BlockPending() { clear(); }
 	void clear()
 	{
-		r.logical_ok = r.frame_ok = r.frame_miss = r.skipped = r.sha256 = r.sha512 = r.frames = 0;
+		r.logical_ok = r.frame_ok = r.frame_miss = r.skipped = r.sha256 = r.sha512 = r.frames = r.lzjb = r.zle = 0;
 		r.first_bad = r.first_miss = ~0ull;
 		obj = off = 0;
 		ctype = 0;
@@ -38,7 +38,8 @@ struct BlockPending {
 };
 
 // device scratch of one codec batch (modes COMPRESS / DECOMPRESS / RECOMPRESS); in VERIFY with
-// MTZ_FLAG_BLOCK_FRAMES the encoder's jobs, scratch and frame sums of the block check (enc, d_enc, osums)
+// MTZ_FLAG_BLOCK_FRAMES / _LZJB the encoders' jobs, scratch and frame sums of the block check (enc, d_enc,
+// osums, k3_skip)
 struct CodecBufs {
 	size_t rec_cap = 0, scratch_cap = 0;
 	CodecRec *cr = nullptr;
@@ -49,6 +50,7 @@ struct CodecBufs {
 	StampStep *steps = nullptr;                         // per-record transitions of the stamp chain
 	uint8_t *d_logical = nullptr, *d_enc = nullptr;
 	uint32_t *seq_n = nullptr, *cert = nullptr;         // RECOMPRESS certificate: K2's parse sizes, K3c's verdicts
+	uint32_t *k3_skip = nullptr;                        // VERIFY with BLOCK_FRAMES and BLOCK_LZJB: K3 leaves these jobs
 	CodecResult *d_cres = nullptr, *h_cres = nullptr;   // h_: pinned
 	ScanResult *d_ores = nullptr, *h_ores = nullptr;    // output-chain result
 	uint64_t *d_outpos = nullptr;                       // running output offset (device)

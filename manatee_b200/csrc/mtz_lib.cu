@@ -308,6 +308,8 @@ int32_t mtz_open(const mtz_config *cfg, mtz_handle **out)
 		return fail(nullptr, MTZ_EINVAL, "BLOCK_SHA512 extends the block check: it needs BLOCK_CKSUM");
 	if ((full.flags & MTZ_FLAG_BLOCK_FRAMES) && !(full.flags & MTZ_FLAG_BLOCK_CKSUM))
 		return fail(nullptr, MTZ_EINVAL, "BLOCK_FRAMES extends the block check: it needs BLOCK_CKSUM");
+	if ((full.flags & MTZ_FLAG_BLOCK_LZJB) && !(full.flags & MTZ_FLAG_BLOCK_CKSUM))
+		return fail(nullptr, MTZ_EINVAL, "BLOCK_LZJB extends the block check: it needs BLOCK_CKSUM");
 	const cudaDeviceProp &prop = props[0];
 
 	mtz_handle *h = new (std::nothrow) mtz_handle();
@@ -318,8 +320,10 @@ int32_t mtz_open(const mtz_config *cfg, mtz_handle **out)
 	// the LZ4 kernels want thousands of records in flight (one warp per record, ~5 ms per
 	// record): measured e2e RECOMPRESS 26 / 41 / 48 / 49 GiB/s logical at 64 / 128 / 256 /
 	// 512 MiB batches; Fletcher alone is happy with 32 MiB batches.  VERIFY with MTZ_FLAG_BLOCK_FRAMES
-	// runs the same encoder over the batch's raw LZ4-keyed records, and wants its records in flight too
-	const bool frames_verify = cfg->mode == MTZ_MODE_VERIFY && (full.flags & MTZ_FLAG_BLOCK_FRAMES);
+	// runs the same encoder over the batch's raw LZ4-keyed records, and wants its records in flight too;
+	// so do the lzjb / zle encoders of MTZ_FLAG_BLOCK_LZJB (one warp per record as well)
+	const bool frames_verify = cfg->mode == MTZ_MODE_VERIFY &&
+	    (full.flags & (MTZ_FLAG_BLOCK_FRAMES | MTZ_FLAG_BLOCK_LZJB));
 	if (h->cfg.batch_bytes == 0)
 		h->cfg.batch_bytes = (codec_mode || frames_verify) ? (256ull << 20) : (32ull << 20);
 	// the input ring holds the batch being filled plus the ones whose H2D copy is still pending
@@ -557,11 +561,19 @@ static int32_t launch_scan(mtz_handle *h, cudaStream_t st, const RecSums *d_sums
 static bool block_on(const mtz_handle *h) { return (h->cfg.flags & MTZ_FLAG_BLOCK_CKSUM) != 0; }
 static bool block_sha256_on(const mtz_handle *h) { return (h->cfg.flags & MTZ_FLAG_BLOCK_SHA256) != 0; }
 static bool block_sha512_on(const mtz_handle *h) { return (h->cfg.flags & MTZ_FLAG_BLOCK_SHA512) != 0; }
-// VERIFY with MTZ_FLAG_BLOCK_FRAMES: the block check encodes frames (kernels_frames.cuh); the other modes
-// accept the flag and have their frames already
+// VERIFY with MTZ_FLAG_BLOCK_FRAMES or MTZ_FLAG_BLOCK_LZJB: the block check encodes frames
+// (kernels_frames.cuh); the other modes accept the flags and encode none
 static bool block_frames_on(const mtz_handle *h)
 {
-	return (h->cfg.flags & MTZ_FLAG_BLOCK_FRAMES) != 0 && h->cfg.mode == MTZ_MODE_VERIFY;
+	return (h->cfg.flags & (MTZ_FLAG_BLOCK_FRAMES | MTZ_FLAG_BLOCK_LZJB)) != 0 && h->cfg.mode == MTZ_MODE_VERIFY;
+}
+static bool block_lzjb_on(const mtz_handle *h) { return (h->cfg.flags & MTZ_FLAG_BLOCK_LZJB) != 0; }
+// block_classify's BLK_FR_* bits: LZ4 frames in VERIFY with MTZ_FLAG_BLOCK_FRAMES (the codec modes have
+// their own), lzjb / zle keys with MTZ_FLAG_BLOCK_LZJB (block_classify limits them to VERIFY and RECOMPRESS)
+static uint32_t block_fcodecs(const mtz_handle *h)
+{
+	return ((h->cfg.flags & MTZ_FLAG_BLOCK_FRAMES) && h->cfg.mode == MTZ_MODE_VERIFY ? BLK_FR_LZ4 : 0u) |
+	    (block_lzjb_on(h) ? BLK_FR_LZJB : 0u);
 }
 static uint32_t block_hashed(const mtz_handle *h)
 {
@@ -588,18 +600,18 @@ static int32_t launch_block(mtz_handle *h, cudaStream_t st, const uint8_t *d_in,
 	const bool sha = block_sha256_on(h), sha512 = block_sha512_on(h);
 	const unsigned grid = (unsigned)((nrec + BLK_THREADS - 1) / BLK_THREADS);
 	k_block_check<<<grid, BLK_THREADS, 0, st>>>(d_in, d_recs, isums, orecs, osums, (uint32_t)nrec,
-	    h->cfg.mode, base, bres, block_hashed(h), fjobs);
+	    h->cfg.mode, base, bres, block_hashed(h), fjobs, block_fcodecs(h));
 	MTZ_CU(h, cudaGetLastError());
 	if (sha) {
 		const unsigned gs = (unsigned)((nrec + SHA_THREADS - 1) / SHA_THREADS);
 		k_block_sha256<<<gs, SHA_THREADS, 0, st>>>(d_in, d_recs, d_out, orecs, (uint32_t)nrec, h->cfg.mode,
-		    base, bres, fjobs);
+		    base, bres, fjobs, block_fcodecs(h));
 		MTZ_CU(h, cudaGetLastError());
 	}
 	if (sha512) {
 		const unsigned gs = (unsigned)((nrec + SHA512_THREADS - 1) / SHA512_THREADS);
 		k_block_sha512<<<gs, SHA512_THREADS, 0, st>>>(d_in, d_recs, d_out, orecs, (uint32_t)nrec, h->cfg.mode,
-		    base, bres, fjobs);
+		    base, bres, fjobs, block_fcodecs(h));
 		MTZ_CU(h, cudaGetLastError());
 	}
 	return MTZ_OK;
@@ -608,8 +620,10 @@ static int32_t launch_block(mtz_handle *h, cudaStream_t st, const uint8_t *d_in,
 static int32_t launch_k3(mtz_handle *h, cudaStream_t st, const void *d_src, void *d_dst,
     mtz_job *d_jobs, uint32_t njobs, bool compact, const uint32_t *skip = nullptr, bool count = true);
 
-// The block check of a VERIFY (sub-)batch with MTZ_FLAG_BLOCK_FRAMES: plan, K3 and the frame sums into
-// cb's jobs / scratch / osums (kernels_frames.cuh), then launch_block against those frames.  The
+// The block check of a VERIFY (sub-)batch with MTZ_FLAG_BLOCK_FRAMES and/or MTZ_FLAG_BLOCK_LZJB: plan,
+// K3 (LZ4 jobs, with BLOCK_FRAMES), k_lzjb_encode and k_zle_encode (lzjb / zle jobs, with BLOCK_LZJB)
+// and the frame sums into cb's jobs / scratch / osums (kernels_frames.cuh), then launch_block against
+// those frames.  The
 // headers of records [0, nrec) lie at d_in + rec.off with rec.off - base_off < cb.scratch_cap
 // (base_off 16-aligned); `compact` as for COMPRESS (all_compact_blocks).  Like the rest of the check,
 // nothing here is counted in mtz_stats.
@@ -620,11 +634,22 @@ static int32_t launch_block_frames(mtz_handle *h, cudaStream_t st, CodecBufs &cb
 	if (nrec == 0) return MTZ_OK;
 	if (nrec > cb.rec_cap) return fail(h, MTZ_ENOSPC, "frame batch of %zu records exceeds %zu", nrec, cb.rec_cap);
 	const uint32_t n = (uint32_t)nrec;
+	const uint32_t fc = block_fcodecs(h);
+	uint32_t *k3_skip = (fc & BLK_FR_LZ4) && (fc & BLK_FR_LZJB) ? cb.k3_skip : nullptr;
 	k_frame_plan<<<(n + FRP_THREADS - 1) / FRP_THREADS, FRP_THREADS, 0, st>>>(d_in, d_recs, n, block_hashed(h),
-	    base_off, cb.d_enc, cb.enc);
+	    base_off, cb.d_enc, cb.enc, fc, k3_skip);
 	MTZ_CU(h, cudaGetLastError());
-	int32_t rc = launch_k3(h, st, nullptr, nullptr, cb.enc, n, compact, nullptr, false);
-	if (rc != MTZ_OK) return rc;
+	if (fc & BLK_FR_LZ4) {
+		const int32_t rc = launch_k3(h, st, nullptr, nullptr, cb.enc, n, compact, k3_skip, false);
+		if (rc != MTZ_OK) return rc;
+	}
+	if (fc & BLK_FR_LZJB) {
+		const unsigned gl = (unsigned)std::min<size_t>((nrec + LZJB_WARPS - 1) / LZJB_WARPS, (size_t)h->sm_count * 8);
+		k_lzjb_encode<<<gl, LZJB_THREADS, 0, st>>>(cb.enc, n);
+		MTZ_CU(h, cudaGetLastError());
+		k_zle_encode<<<gl, LZJB_THREADS, 0, st>>>(cb.enc, n);
+		MTZ_CU(h, cudaGetLastError());
+	}
 	const unsigned gs = (unsigned)std::min<size_t>((nrec + K1_WARPS - 1) / K1_WARPS, (size_t)h->sm_count * 16);
 	k_frame_sums<<<gs, K1_THREADS, 0, st>>>(cb.enc, n, cb.osums, bres);
 	MTZ_CU(h, cudaGetLastError());
@@ -639,7 +664,7 @@ static int32_t block_take(mtz_handle *h, BlockPending &p, const BlockResult &r, 
 {
 	p.r.logical_ok += r.logical_ok; p.r.frame_ok += r.frame_ok;
 	p.r.frame_miss += r.frame_miss; p.r.skipped += r.skipped; p.r.sha256 += r.sha256;
-	p.r.sha512 += r.sha512; p.r.frames += r.frames;
+	p.r.sha512 += r.sha512; p.r.frames += r.frames; p.r.lzjb += r.lzjb; p.r.zle += r.zle;
 	p.r.first_miss = std::min(p.r.first_miss, r.first_miss);
 	if (r.first_bad < p.r.first_bad) {
 		uint64_t w[6];      // header bytes 8..55: drr_object, drr_offset, drr_checksumtype
@@ -663,6 +688,7 @@ static int32_t block_fold(mtz_handle *h, BlockPending &p, uint64_t stream_bad)
 		h->bstats.frame_miss += q.r.frame_miss; h->bstats.skipped += q.r.skipped;
 		h->bstats.sha256 += q.r.sha256; h->bstats.sha512 += q.r.sha512;
 		h->bstats.frames_encoded += q.r.frames;
+		h->bstats.lzjb_encoded += q.r.lzjb; h->bstats.zle_encoded += q.r.zle;
 		h->bstats.first_frame_miss = std::min<uint64_t>(h->bstats.first_frame_miss, q.r.first_miss);
 	}
 	if (q.r.first_bad == ~0ull || q.r.first_bad >= stream_bad) return MTZ_OK;
@@ -727,6 +753,8 @@ static int32_t codec_alloc(mtz_handle *h, CodecBufs &cb, size_t rec_cap, size_t 
 	if (h->cfg.mode == MTZ_MODE_DECOMPRESS || h->cfg.mode == MTZ_MODE_RECOMPRESS)
 		MTZ_CU(h, cudaMalloc(&cb.d_logical, scratch_cap + 512));
 	if (h->cfg.mode != MTZ_MODE_DECOMPRESS) MTZ_CU(h, cudaMalloc(&cb.d_enc, scratch_cap + 512));
+	if (h->cfg.mode == MTZ_MODE_VERIFY && block_lzjb_on(h) && (h->cfg.flags & MTZ_FLAG_BLOCK_FRAMES))
+		MTZ_CU(h, cudaMalloc(&cb.k3_skip, rec_cap * sizeof(uint32_t)));
 	if (certify_on(h)) {
 		MTZ_CU(h, cudaMalloc(&cb.seq_n, rec_cap * sizeof(uint32_t)));
 		MTZ_CU(h, cudaMalloc(&cb.cert, rec_cap * sizeof(uint32_t)));
@@ -745,7 +773,7 @@ static void codec_free(CodecBufs &cb)
 	cudaFree(cb.cr); cudaFree(cb.vals); cudaFree(cb.offs); cudaFree(cb.out_offs);
 	cudaFree(cb.dec); cudaFree(cb.enc); cudaFree(cb.out_recs); cudaFree(cb.osums); cudaFree(cb.steps);
 	cudaFree(cb.d_logical); cudaFree(cb.d_enc); cudaFree(cb.d_cres); cudaFree(cb.d_ores);
-	cudaFree(cb.d_outpos); cudaFree(cb.seq_n); cudaFree(cb.cert);
+	cudaFree(cb.d_outpos); cudaFree(cb.seq_n); cudaFree(cb.cert); cudaFree(cb.k3_skip);
 	if (cb.h_cres) cudaFreeHost(cb.h_cres);
 	if (cb.h_ores) cudaFreeHost(cb.h_ores);
 	cb = CodecBufs();
@@ -941,7 +969,7 @@ static int32_t dv_host_recs(mtz_handle *h, cudaStream_t st, const mtz_rec *d_rec
 	return MTZ_OK;
 }
 
-// The block check of a VERIFY submit with MTZ_FLAG_BLOCK_FRAMES, in sub-batches whose input span fits
+// The block check of a VERIFY submit with MTZ_FLAG_BLOCK_FRAMES / _LZJB, in sub-batches whose input span fits
 // dv_cb's scratch (2 GiB) and whose records fit its tables; one after another on `st`, verdicts into
 // dv_bres for the finish.
 static int32_t dv_block_frames(mtz_handle *h, cudaStream_t st, const uint8_t *d_in, const mtz_rec *d_recs,

@@ -123,7 +123,8 @@ class ZfsClient(object):
                                 block_checksums=bool(g.get("blockChecksums")),
                                 block_sha256=bool(g.get("blockSha256")),
                                 block_sha512=bool(g.get("blockSha512")),
-                                block_frames=bool(g.get("blockFrames")))
+                                block_frames=bool(g.get("blockFrames")),
+                                block_lzjb=bool(g.get("blockLzjb")))
 
     def _wire_mode(self, serverUrl, jobPath):
         """Which stage to put in the pipe for THIS job (SURVEY.md 8f f2).  A receiver configured

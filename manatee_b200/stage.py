@@ -21,7 +21,7 @@ class GpuSnapshotStage(object):
 
     def __init__(self, mode="verify", device=0, ring_bytes=0, batch_bytes=0, n_slots=0,
                  out_ring_bytes=0, flags=0, devices=None, block_checksums=False, block_sha256=False,
-                 block_sha512=False, block_frames=False):
+                 block_sha512=False, block_frames=False, block_lzjb=False):
         """``devices`` = CUDA ordinals of a device group: the GPUs of one box run as ONE stage,
         batch b of the stream on ``devices[b % len(devices)]`` (mtz_config.devices[]).
         ``block_checksums`` = MTZ_FLAG_BLOCK_CKSUM: every DRR_WRITE is also checked against the
@@ -33,7 +33,11 @@ class GpuSnapshotStage(object):
         ``block_frames`` = MTZ_FLAG_BLOCK_FRAMES: in VERIFY, a block that arrives raw while its key
         covers an LZ4 frame on disk is compared with the stage's encoder frame of it instead of
         being skipped (``block_stats()["frames_encoded"]``); the other modes accept it and do not
-        change.  Only valid with ``block_checksums``."""
+        change.  Only valid with ``block_checksums``.
+        ``block_lzjb`` = MTZ_FLAG_BLOCK_LZJB: keys over an lzjb or zle frame on disk are checked too:
+        a record that arrives as that frame (VERIFY, RECOMPRESS) as it is, a raw one in VERIFY
+        against the stage's lzjb / zle encoder frame of it (``block_stats()["lzjb_encoded"]``,
+        ``["zle_encoded"]``).  With or without ``block_frames``; only valid with ``block_checksums``."""
         if block_checksums:
             flags |= N.FLAG_BLOCK_CKSUM
         if block_sha256:
@@ -42,6 +46,8 @@ class GpuSnapshotStage(object):
             flags |= N.FLAG_BLOCK_SHA512
         if block_frames:
             flags |= N.FLAG_BLOCK_FRAMES
+        if block_lzjb:
+            flags |= N.FLAG_BLOCK_LZJB
         self._L = N.lib()
         self._h = C.c_void_p()
         cfg = N.Config()

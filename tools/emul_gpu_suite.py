@@ -39,12 +39,17 @@ PARAMS = {
                                                                         (False, True), (True, True)],
     "test_lz4_on_disk_keys_match_the_encoder_in_verify": [(9, 512), (9, 8192), (12, 8192), (12, 131072)],
     "test_sha256_and_sha512_lz4_on_disk_keys": [(9,), (12,)],
+    "test_lzjb_and_zle_keys_match_the_encoders_in_verify": [(512, 9, False), (8192, 9, False), (8192, 12, True),
+                                                            (131072, 9, True)],
+    "test_sha256_and_sha512_keys": [("sha256",), ("sha512",)],
+    "test_send_c_stream_frames_checked_as_they_arrive": [("verify",), ("recompress",)],
 }
 SKIP = {"test_sixteen_mib_record": "16 MiB blocks take minutes per encode on the emulator",
         "test_size_independent_properties_at_2gib": "2 GiB of LZ4 work is out of reach for the emulator",
         "test_device_api_across_the_subbatch_edge": "66 000 records; tests/test_emul_block_cksum.py crosses the "
                                                     "emulated build's 700-record edge instead",
-        "test_device_group": "needs two GPUs"}
+        "test_device_group": "needs two GPUs",
+        "test_real_streams_with_lzjb_or_zle_keys": "tests/golden/real holds no stream with lzjb or zle keys"}
 
 
 def main():
@@ -61,12 +66,13 @@ def main():
     import test_gpu_block_sha256 as H
     import test_gpu_block_sha512 as W
     import test_gpu_block_frames as F
+    import test_gpu_block_lzjb as J
     import test_gpu_codec as K
     import test_gpu_lz4 as Z
     import test_gpu_stream as S
     import test_gpu_verify as V
     tot = fail = 0
-    for mod in (V, S, Z, K, B, H, W, F):
+    for mod in (V, S, Z, K, B, H, W, F, J):
         for name, fn in inspect.getmembers(mod, inspect.isfunction):
             if not name.startswith("test_") or filt not in name:
                 continue
