@@ -29,15 +29,19 @@ namespace mtz {
 #define BLK_FR_LZJB    2u      // MTZ_FLAG_BLOCK_LZJB: lzjb and zle frames, and in VERIFY and
                                // RECOMPRESS lzjb / zle records that arrive as their disk frame
 
+// The counters carry their mtz_block_stats names.
 struct BlockResult {           // device, mirrored to pinned host; zeroed per batch
 	unsigned long long logical_ok, frame_ok, frame_miss, skipped;
 	unsigned long long sha256;       // records compared by k_block_sha256 (kernels_sha256.cuh)
 	unsigned long long sha512;       // records compared by k_block_sha512 (kernels_sha512.cuh)
-	unsigned long long frames;       // LZ4 frames encoded for the check (k_frame_sums, kernels_frames.cuh)
-	unsigned long long lzjb, zle;    // lzjb / zle frames encoded for the check (likewise)
-	unsigned long long first_bad;    // stream index of the first logical mismatch, ~0 none
-	unsigned long long first_miss;   // stream index of the first frame mismatch, ~0 none
+	unsigned long long frames_encoded;   // LZ4 frames encoded for the check (k_frame_sums, kernels_frames.cuh)
+	unsigned long long lzjb_encoded, zle_encoded;   // lzjb / zle frames encoded for the check (likewise)
+	unsigned long long first_bad;          // stream index of the first logical mismatch, ~0 none
+	unsigned long long first_frame_miss;   // stream index of the first frame mismatch, ~0 none
 };
+// a batch's results are reset by zeroing everything before first_bad and setting the rest to ~0
+static_assert(offsetof(BlockResult, first_frame_miss) == offsetof(BlockResult, first_bad) + 8 &&
+    sizeof(BlockResult) == offsetof(BlockResult, first_frame_miss) + 8, "first_bad, first_frame_miss: last");
 
 // zero-state sums of a segment's tail, given the sums of the whole segment and of its 8-word head
 // (the inverse of apply(head, tail) for a tail of n words)
@@ -101,24 +105,78 @@ __device__ __forceinline__ void block_verdict(BlockResult *res, int what, bool o
 		atomicAdd(&res->frame_ok, 1ull);
 	} else {
 		atomicAdd(&res->frame_miss, 1ull);
-		atomicMin(&res->first_miss, (unsigned long long)idx);
+		atomicMin(&res->first_frame_miss, (unsigned long long)idx);
 	}
 }
 
+// The key types checked at all: fletcher4, and type t where `hashed` has bit t set (bit 8:
+// k_block_sha256 with MTZ_FLAG_BLOCK_SHA256, bit 11: k_block_sha512 with MTZ_FLAG_BLOCK_SHA512).
+__device__ __forceinline__ bool block_key_checked(uint32_t t, uint32_t hashed)
+{
+	return t == ZIO_CKSUM_FLETCHER4 || (t < 32u && ((hashed >> t) & 1u));
+}
+
+// block_classify for the kernels below.  `orecs`: the output records of a re-encoding mode, else
+// null.  `have_out` is read only in COMPRESS, DECOMPRESS and RECOMPRESS, where codec_launch_post
+// passes the output records together with their sums: `orecs != nullptr` is `osums != nullptr` there.
+__device__ __forceinline__ BlockClass block_class(const uint8_t *hdr, const mtz_rec &rec, uint32_t mode,
+    uint32_t ctype, uint32_t frames, const mtz_rec *orecs)
+{
+	return block_classify(hdr, rec, mode, orecs != nullptr, ctype, frames);
+}
+
+// Record r's key of type `ctype` against the bytes block_classify picks: the input payload, output
+// record r (at `d_out` + its offset) or VERIFY's frame job r (`fjobs`, kernels_frames.cuh), `nbytes`
+// of them at `p`, zero-extended to `cover`.  The stage's encoder storing the block raw where ZFS's
+// stored a frame (not that encoder) and bytes longer than the key covers are mismatches;
+// `match(p, nbytes, cover, src)` compares the rest.  The verdict goes to `res` as stream record
+// `base + r`, after a bump of res->*counter (null: none).  False: a key this kernel does not check.
+template <class Match>
+__device__ __forceinline__ bool block_compare(const uint8_t *hdr, const mtz_rec &rec, uint32_t r, uint32_t mode,
+    uint32_t ctype, uint32_t frames, const mtz_rec *orecs, const uint8_t *d_out, const mtz_job *fjobs,
+    BlockResult *res, uint64_t base, unsigned long long BlockResult::*counter, Match match)
+{
+	const BlockClass c = block_class(hdr, rec, mode, ctype, frames, orecs);
+	if (c.what == 0) return false;
+	const uint8_t *p;
+	uint64_t nbytes;
+	bool ok = true;
+	if (c.src == 0) {
+		p = hdr + DRR_HDR;
+		nbytes = (uint64_t)rec.payload;
+	} else if (fjobs == nullptr) {
+		const mtz_rec o = orecs[r];
+		p = d_out + o.off + DRR_HDR;
+		nbytes = (uint64_t)o.payload;
+		if (c.what == 2 && o.comp != ZIO_LZ4) ok = false;
+	} else {
+		const mtz_job j = fjobs[r];
+		p = reinterpret_cast<const uint8_t *>((uintptr_t)j.dst_off);
+		nbytes = (uint64_t)j.out_len;
+		if (j.out_len >= rec.lsize) ok = false;      // stored raw
+	}
+	const uint64_t cover = (c.what == 1) ? c.lsz : c.psz;
+	if (nbytes > cover) ok = false;
+	if (ok) ok = match(p, nbytes, cover, c.src);
+	if (counter != nullptr) atomicAdd(&(res->*counter), 1ull);
+	block_verdict(res, c.what, ok, base + r);
+	return true;
+}
+
 // One thread per record.  `isums` are the input's K1 sums (body from byte 280), `orecs`/`osums`
-// the output records and their payload sums in the re-encoding modes (null in VERIFY).  Record r
-// is record `base + r` of the stream.  `hashed` has bit t set for each key type t another kernel
-// hashes (bit 8: k_block_sha256 with MTZ_FLAG_BLOCK_SHA256, bit 11: k_block_sha512 with
-// MTZ_FLAG_BLOCK_SHA512): the keys of those types this stage can check are left to that kernel
-// instead of being counted as skipped.  `fjobs` (VERIFY with MTZ_FLAG_BLOCK_FRAMES or
-// MTZ_FLAG_BLOCK_LZJB, else null): the frame jobs of kernels_frames.cuh, whose frames stand in for the
-// output records and whose sums are in `osums`.  `frames`: block_classify's BLK_FR_* bits.
+// the output records and their payload sums in the re-encoding modes (null in VERIFY), `d_out` the
+// output batch the offsets of `orecs` refer to.  Record r is record `base + r` of the stream.
+// `hashed` as block_key_checked's: the keys of those types this stage can check are left to the
+// kernel that hashes them instead of being counted as skipped.  `fjobs` (VERIFY with
+// MTZ_FLAG_BLOCK_FRAMES or MTZ_FLAG_BLOCK_LZJB, else null): the frame jobs of kernels_frames.cuh,
+// whose frames stand in for the output records and whose sums are in `osums`.  `frames`:
+// block_classify's BLK_FR_* bits.
 #define BLK_THREADS 128
 __global__ void __launch_bounds__(BLK_THREADS)
 k_block_check(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs,
     const RecSums *__restrict__ isums, const mtz_rec *__restrict__ orecs,
-    const RecSums *__restrict__ osums, uint32_t n, uint32_t mode, uint64_t base,
-    BlockResult *__restrict__ res, uint32_t hashed, const mtz_job *__restrict__ fjobs = nullptr,
+    const RecSums *__restrict__ osums, const uint8_t *__restrict__ d_out, uint32_t n, uint32_t mode,
+    uint64_t base, BlockResult *__restrict__ res, uint32_t hashed, const mtz_job *__restrict__ fjobs = nullptr,
     uint32_t frames = 0u)
 {
 	const uint32_t r = blockIdx.x * BLK_THREADS + threadIdx.x;
@@ -126,38 +184,23 @@ k_block_check(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs
 	const mtz_rec rec = recs[r];
 	if (rec.type != DRR_WRITE_T) return;
 	const uint8_t *hdr = d_in + rec.off;
-	const BlockClass c = block_classify(hdr, rec, mode, osums != nullptr, ZIO_CKSUM_FLETCHER4, frames);
-	const int what = c.what, src = c.src;
-	if (what == 0) {
+	const bool checked = block_compare(hdr, rec, r, mode, ZIO_CKSUM_FLETCHER4, frames, orecs, d_out, fjobs, res,
+	    base, nullptr, [&](const uint8_t *, uint64_t nbytes, uint64_t cover, int src) {
+		Ck4 sums;
+		if (src == 0) {
+			const RecSums s = isums[r];
+			const Ck4 zero = { 0, 0, 0, 0 };
+			sums = strip_head8(s.body, fold_cksum_words(zero, s.emb), s.nbody - 8u);
+		} else {
+			sums = osums[r].body;
+		}
+		return ck_eq(shift_zeros(sums, (cover - nbytes) >> 2), load_ck(hdr + 56));
+	});
+	if (!checked) {
 		const uint32_t t = hdr[48];
-		if (t >= 32u || !((hashed >> t) & 1u) || block_classify(hdr, rec, mode, osums != nullptr, t, frames).what == 0)
+		if (!block_key_checked(t, hashed) || block_class(hdr, rec, mode, t, frames, orecs).what == 0)
 			atomicAdd(&res->skipped, 1ull);
-		return;
 	}
-	Ck4 sums;
-	uint64_t nbytes;
-	bool ok = true;
-	if (src == 0) {
-		const RecSums s = isums[r];
-		const Ck4 zero = { 0, 0, 0, 0 };
-		nbytes = (uint64_t)rec.payload;
-		sums = strip_head8(s.body, fold_cksum_words(zero, s.emb), s.nbody - 8u);
-	} else if (fjobs == nullptr) {
-		const mtz_rec o = orecs[r];
-		nbytes = (uint64_t)o.payload;
-		sums = osums[r].body;
-		// the stage's encoder stored the block raw where ZFS's stored a frame: not that encoder
-		if (what == 2 && o.comp != ZIO_LZ4) ok = false;
-	} else {
-		const mtz_job j = fjobs[r];
-		nbytes = (uint64_t)j.out_len;
-		sums = osums[r].body;
-		if (j.out_len >= rec.lsize) ok = false;      // stored raw: likewise
-	}
-	const uint64_t cover = (what == 1) ? c.lsz : c.psz;
-	if (nbytes > cover) ok = false;
-	if (ok) ok = ck_eq(shift_zeros(sums, (cover - nbytes) >> 2), load_ck(hdr + 56));
-	block_verdict(res, what, ok, base + r);
 }
 
 } // namespace mtz

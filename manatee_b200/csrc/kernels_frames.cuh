@@ -20,8 +20,8 @@ namespace mtz {
 // Record r's slot is scratch + (rec.off & ~15) - base_off: its frame is at most lsize bytes and the
 // record itself spans 312 + lsize bytes of the batch, so the slots of a batch do not overlap and
 // the scratch needs no more bytes than the batch (base_off 16-aligned, at or before the first
-// header).  `hashed` as k_block_check's: the key types checked besides fletcher4; `frames`:
-// block_classify's BLK_FR_* bits.  A job's src_len is its codec (BLK_DC_LZ4 / _LZJB / _ZLE).
+// header).  `hashed` as block_key_checked's; `frames`: block_classify's BLK_FR_* bits.  A job's
+// src_len is its codec (BLK_DC_LZ4 / _LZJB / _ZLE).
 // `k3_skip` (null unless both flags are on): 1 for each job K3 must leave to the other encoders.
 #define FRP_THREADS 128
 __global__ void __launch_bounds__(FRP_THREADS)
@@ -37,7 +37,7 @@ k_frame_plan(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs,
 	if (rec.type == DRR_WRITE_T) {
 		const uint8_t *hdr = d_in + rec.off;
 		const uint32_t t = hdr[48];
-		if (t == ZIO_CKSUM_FLETCHER4 || (t < 32u && ((hashed >> t) & 1u))) {
+		if (block_key_checked(t, hashed)) {
 			const BlockClass c = block_classify(hdr, rec, MTZ_MODE_VERIFY, false, t, frames);
 			if (c.what == 2 && c.src == 1) {
 				j.src_len = (uint32_t)((*reinterpret_cast<const uint64_t *>(hdr + 88) >> 32) & 0x7full);
@@ -52,8 +52,9 @@ k_frame_plan(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs,
 }
 
 // One warp per record (grid-stride): zero-state sums of the frame its encoder left at jobs[r].dst_off
-// into sums[r].body, and the record counted in res->frames, res->lzjb or res->zle by its codec.  A frame the encoder stored raw (out_len ==
-// lsize) has no sums: the checks count it as a miss without reading them.
+// into sums[r].body, and the record counted in res->frames_encoded, lzjb_encoded or zle_encoded by its
+// codec.  A frame the encoder stored raw (out_len == lsize) has no sums: the checks count it as a
+// miss without reading them.
 __global__ void __launch_bounds__(K1_THREADS)
 k_frame_sums(const mtz_job *__restrict__ jobs, uint32_t n, RecSums *__restrict__ sums,
     BlockResult *__restrict__ res)
@@ -79,7 +80,8 @@ k_frame_sums(const mtz_job *__restrict__ jobs, uint32_t n, RecSums *__restrict__
 		}
 		if (lane == 0) {
 			sums[r].body = acc;
-			atomicAdd(j.src_len == BLK_DC_LZJB ? &res->lzjb : j.src_len == BLK_DC_ZLE ? &res->zle : &res->frames, 1ull);
+			atomicAdd(j.src_len == BLK_DC_LZJB ? &res->lzjb_encoded : j.src_len == BLK_DC_ZLE ? &res->zle_encoded :
+			    &res->frames_encoded, 1ull);
 		}
 	}
 }

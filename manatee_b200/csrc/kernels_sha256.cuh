@@ -65,98 +65,119 @@ __device__ __forceinline__ void sha256_compress(uint32_t st[8], uint32_t w[16])
 	st[4] += e; st[5] += f; st[6] += g; st[7] += h;
 }
 
+__device__ __forceinline__ uint64_t sha_join(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
+// the big-endian u64 of 8 bytes loaded as a little-endian uint2 (also: bswap64 of sha_join(x, y))
+__device__ __forceinline__ uint64_t sha_be64(uint2 v) { return sha_join(sha_be32(v.y), sha_be32(v.x)); }
+
 // Block k of the message "nbytes of `p`, zeros up to `cover`, FIPS 180-4 padding" as 16 big-endian
-// words.  `p` is 8-byte aligned, `nbytes` a multiple of 8; no byte at or past p[nbytes] is read (the
-// zeros are arithmetic).
-__device__ __forceinline__ void sha256_message_block(const uint8_t *__restrict__ p, uint64_t nbytes,
-    uint64_t cover, uint64_t k, uint32_t w[16])
+// words W: SHA-256's 64-byte blocks of 32-bit words, SHA-512's 128-byte blocks of 64-bit words.
+// `p` is 8-byte aligned, `nbytes` a multiple of 8, `cover` a multiple of the block; no byte at or
+// past p[nbytes] is read (the zeros are arithmetic).
+template <class W>
+__device__ __forceinline__ void sha_message_block(const uint8_t *__restrict__ p, uint64_t nbytes,
+    uint64_t cover, uint64_t k, W w[16])
 {
-	const uint64_t o = k * 64ull;
-	if (o + 64ull <= nbytes) {
+	constexpr uint64_t block = 16 * sizeof(W);
+	const uint64_t o = k * block;
+	auto put = [&](int i, uint2 v) {      // chunk i: 8 bytes
+		if constexpr (sizeof(W) == 4) {
+			w[2 * i] = sha_be32(v.x); w[2 * i + 1] = sha_be32(v.y);
+		} else {
+			w[i] = sha_be64(v);
+		}
+	};
+	if (o + block <= nbytes) {
 		const uint2 *q = reinterpret_cast<const uint2 *>(p + o);
 #pragma unroll
-		for (int i = 0; i < 8; i++) {
-			const uint2 v = q[i];
-			w[2 * i] = sha_be32(v.x); w[2 * i + 1] = sha_be32(v.y);
-		}
+		for (int i = 0; i < (int)block / 8; i++) put(i, q[i]);
 	} else if (o < nbytes) {
 		// the block where the payload ends and the zero extension begins (payload lengths are
 		// multiples of 8: the parsers reject anything else)
 		const uint64_t rem = nbytes - o;
 #pragma unroll
-		for (int i = 0; i < 8; i++) {
+		for (int i = 0; i < (int)block / 8; i++) {
 			uint2 v = make_uint2(0u, 0u);
 			if (8ull * (uint64_t)i < rem) v = reinterpret_cast<const uint2 *>(p + o)[i];
-			w[2 * i] = sha_be32(v.x); w[2 * i + 1] = sha_be32(v.y);
+			put(i, v);
 		}
 	} else {
 #pragma unroll
 		for (int i = 0; i < 16; i++) w[i] = 0u;
 		if (o >= cover) {
 			const uint64_t bits = cover * 8ull;
-			w[0] = 0x80000000u;
-			w[14] = (uint32_t)(bits >> 32); w[15] = (uint32_t)bits;
+			w[0] = (W)1 << (8 * sizeof(W) - 1);
+			w[15] = (W)bits;      // SHA-512: the 128-bit length, its high word w[14] stays zero
+			if constexpr (sizeof(W) == 4) w[14] = (W)(bits >> 32);
 		}
 	}
 }
 
-// One thread per record of the (sub-)batch, the same arguments as k_block_check plus the output
-// batch base (`orecs[r].off` is relative to `d_out`).  A record whose key is not a sha256 key this
-// stage can check returns at once; k_block_check counted it or left it to this kernel.
+// The body of k_block_sha256 and k_block_sha512: one thread per record of the (sub-)batch, its key
+// compared (block_compare) with the hash H of its bytes, the records compared counted in
+// res->*H::counter.  A record whose key is not an H key this stage can check returns at once;
+// k_block_check counted it or left it to this kernel.
+template <class H>
+__device__ __forceinline__ void block_sha(const uint8_t *d_in, const mtz_rec *recs, const uint8_t *d_out,
+    const mtz_rec *orecs, uint32_t n, uint32_t mode, uint64_t base, BlockResult *res, const mtz_job *fjobs,
+    uint32_t frames)
+{
+	const uint32_t r = blockIdx.x * H::threads + threadIdx.x;
+	if (r >= n) return;
+	const mtz_rec rec = recs[r];
+	if (rec.type != DRR_WRITE_T) return;
+	const uint8_t *hdr = d_in + rec.off;
+	block_compare(hdr, rec, r, mode, H::ctype, frames, orecs, d_out, fjobs, res, base, H::counter,
+	    [&](const uint8_t *p, uint64_t nbytes, uint64_t cover, int) {
+		typename H::word st[8];
+#pragma unroll
+		for (int i = 0; i < 8; i++) st[i] = H::iv(i);
+		const uint64_t nblk = cover / (16 * sizeof(st[0])) + 1ull;
+		typename H::word cur[16], nxt[16];
+		sha_message_block(p, nbytes, cover, 0, cur);
+		for (uint64_t k = 0; k < nblk; k++) {
+			if (k + 1ull < nblk) sha_message_block(p, nbytes, cover, k + 1ull, nxt);
+			H::compress(st, cur);
+#pragma unroll
+			for (int i = 0; i < 16; i++) cur[i] = nxt[i];
+		}
+		const uint64_t *key = reinterpret_cast<const uint64_t *>(hdr + 56);
+		bool ok = true;
+#pragma unroll
+		for (int i = 0; i < 4; i++)
+			ok = ok && key[i] == H::key_word(st, i);
+		return ok;
+	});
+}
+
+// block_sha's traits for sha256 keys
 #define SHA_THREADS 64
+struct Sha256H {
+	typedef uint32_t word;
+	static constexpr int threads = SHA_THREADS;
+	static constexpr uint32_t ctype = ZIO_CKSUM_SHA256;
+	static constexpr unsigned long long BlockResult::*counter = &BlockResult::sha256;
+	static __device__ __forceinline__ uint32_t iv(int i)      // folds to an immediate for a constant i
+	{
+		const uint32_t v[8] = { 0x6a09e667u, 0xbb67ae85u, 0x3c6ef372u, 0xa54ff53au,
+		                        0x510e527fu, 0x9b05688cu, 0x1f83d9abu, 0x5be0cd19u };
+		return v[i];
+	}
+	static __device__ __forceinline__ void compress(uint32_t st[8], uint32_t w[16]) { sha256_compress(st, w); }
+	// key word i: the digest's bytes 8i..8i+8 big-endian
+	static __device__ __forceinline__ uint64_t key_word(const uint32_t st[8], int i)
+	{
+		return ((uint64_t)st[2 * i] << 32) | st[2 * i + 1];
+	}
+};
+
+// The same arguments as k_block_check's but the sums: the hash reads the bytes
 __global__ void __launch_bounds__(SHA_THREADS)
 k_block_sha256(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs,
     const uint8_t *__restrict__ d_out, const mtz_rec *__restrict__ orecs, uint32_t n, uint32_t mode,
     uint64_t base, BlockResult *__restrict__ res, const mtz_job *__restrict__ fjobs = nullptr,
     uint32_t frames = 0u)
 {
-	const uint32_t r = blockIdx.x * SHA_THREADS + threadIdx.x;
-	if (r >= n) return;
-	const mtz_rec rec = recs[r];
-	if (rec.type != DRR_WRITE_T) return;
-	const uint8_t *hdr = d_in + rec.off;
-	const BlockClass c = block_classify(hdr, rec, mode, orecs != nullptr, ZIO_CKSUM_SHA256, frames);
-	if (c.what == 0) return;
-	const uint8_t *p;
-	uint64_t nbytes;
-	bool ok = true;
-	if (c.src == 0) {
-		p = hdr + DRR_HDR;
-		nbytes = (uint64_t)rec.payload;
-	} else if (fjobs == nullptr) {
-		const mtz_rec o = orecs[r];
-		p = d_out + o.off + DRR_HDR;
-		nbytes = (uint64_t)o.payload;
-		// the stage's encoder stored the block raw where ZFS's stored a frame: not that encoder
-		if (c.what == 2 && o.comp != ZIO_LZ4) ok = false;
-	} else {
-		// VERIFY with MTZ_FLAG_BLOCK_FRAMES / _LZJB: the declared encoder's frame (kernels_frames.cuh)
-		const mtz_job j = fjobs[r];
-		p = reinterpret_cast<const uint8_t *>((uintptr_t)j.dst_off);
-		nbytes = (uint64_t)j.out_len;
-		if (j.out_len >= rec.lsize) ok = false;
-	}
-	const uint64_t cover = (c.what == 1) ? c.lsz : c.psz;
-	if (nbytes > cover) ok = false;
-	if (ok) {
-		uint32_t st[8] = { 0x6a09e667u, 0xbb67ae85u, 0x3c6ef372u, 0xa54ff53au,
-		                   0x510e527fu, 0x9b05688cu, 0x1f83d9abu, 0x5be0cd19u };
-		const uint64_t nblk = cover / 64ull + 1ull;
-		uint32_t cur[16], nxt[16];
-		sha256_message_block(p, nbytes, cover, 0, cur);
-		for (uint64_t k = 0; k < nblk; k++) {
-			if (k + 1ull < nblk) sha256_message_block(p, nbytes, cover, k + 1ull, nxt);
-			sha256_compress(st, cur);
-#pragma unroll
-			for (int i = 0; i < 16; i++) cur[i] = nxt[i];
-		}
-		const uint64_t *key = reinterpret_cast<const uint64_t *>(hdr + 56);
-#pragma unroll
-		for (int i = 0; i < 4; i++)
-			ok = ok && key[i] == (((uint64_t)st[2 * i] << 32) | st[2 * i + 1]);
-	}
-	atomicAdd(&res->sha256, 1ull);
-	block_verdict(res, c.what, ok, base + r);
+	block_sha<Sha256H>(d_in, recs, d_out, orecs, n, mode, base, res, fjobs, frames);
 }
 
 } // namespace mtz

@@ -48,8 +48,6 @@ __device__ __forceinline__ uint64_t sha512_k(int t)
 	return k[t];
 }
 
-__device__ __forceinline__ uint64_t sha_join(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
-
 // 64-bit rotate right by a constant n (1..63) as two 32-bit funnel shifts on the halves
 __device__ __forceinline__ uint64_t sha_rotr64(uint64_t x, int n)
 {
@@ -57,9 +55,6 @@ __device__ __forceinline__ uint64_t sha_rotr64(uint64_t x, int n)
 	if (n < 32) return sha_join(__funnelshift_r(lo, hi, n), __funnelshift_r(hi, lo, n));
 	return sha_join(__funnelshift_r(hi, lo, n - 32), __funnelshift_r(lo, hi, n - 32));
 }
-
-// the big-endian u64 of 8 bytes loaded as a little-endian uint2 (also: bswap64 of sha_join(x, y))
-__device__ __forceinline__ uint64_t sha_be64(uint2 v) { return sha_join(sha_be32(v.y), sha_be32(v.x)); }
 
 // FIPS 180-4 SHA-512 compression of one 128-byte block (`w` = its 16 big-endian words, consumed)
 __device__ __forceinline__ void sha512_compress(uint64_t st[8], uint64_t w[16])
@@ -84,97 +79,37 @@ __device__ __forceinline__ void sha512_compress(uint64_t st[8], uint64_t w[16])
 	st[4] += e; st[5] += f; st[6] += g; st[7] += h;
 }
 
-// Block k of the message "nbytes of `p`, zeros up to `cover`, FIPS 180-4 padding" as 16 big-endian
-// words.  `p` is 8-byte aligned, `nbytes` a multiple of 8, `cover` a multiple of 128; no byte at or
-// past p[nbytes] is read (the zeros are arithmetic).
-__device__ __forceinline__ void sha512_message_block(const uint8_t *__restrict__ p, uint64_t nbytes,
-    uint64_t cover, uint64_t k, uint64_t w[16])
-{
-	const uint64_t o = k * 128ull;
-	if (o + 128ull <= nbytes) {
-		const uint2 *q = reinterpret_cast<const uint2 *>(p + o);
-#pragma unroll
-		for (int i = 0; i < 16; i++) w[i] = sha_be64(q[i]);
-	} else if (o < nbytes) {
-		// the block where the payload ends and the zero extension begins
-		const uint64_t rem = nbytes - o;
-#pragma unroll
-		for (int i = 0; i < 16; i++) {
-			uint2 v = make_uint2(0u, 0u);
-			if (8ull * (uint64_t)i < rem) v = reinterpret_cast<const uint2 *>(p + o)[i];
-			w[i] = sha_be64(v);
-		}
-	} else {
-#pragma unroll
-		for (int i = 0; i < 16; i++) w[i] = 0ull;
-		if (o >= cover) {
-			w[0] = 0x8000000000000000ull;
-			w[15] = cover * 8ull;      // the 128-bit length: its high word w[14] stays zero
-		}
-	}
-}
-
-// SHA-512/256 initial hash value (FIPS 180-4 5.3.6.2)
-#define SHA512_256_IV { 0x22312194fc2bf72cull, 0x9f555fa3c84c64c2ull, 0x2393b86b6f53b151ull, \
-                        0x963877195940eabdull, 0x96283ee2a88effe3ull, 0xbe5e1e2553863992ull, \
-                        0x2b0199fc2c85b8aaull, 0x0eb72ddc81c52ca2ull }
-
-// One thread per record of the (sub-)batch, the same arguments as k_block_sha256.  A record whose
-// key is not a sha512 key this stage can check returns at once; k_block_check counted it or left it
-// to this kernel.
+// block_sha's traits for sha512 keys
 #define SHA512_THREADS 64
+struct Sha512H {
+	typedef uint64_t word;
+	static constexpr int threads = SHA512_THREADS;
+	static constexpr uint32_t ctype = ZIO_CKSUM_SHA512;
+	static constexpr unsigned long long BlockResult::*counter = &BlockResult::sha512;
+	// SHA-512/256 initial hash value (FIPS 180-4 5.3.6.2)
+	static __device__ __forceinline__ uint64_t iv(int i)      // folds to an immediate for a constant i
+	{
+		const uint64_t v[8] = { 0x22312194fc2bf72cull, 0x9f555fa3c84c64c2ull, 0x2393b86b6f53b151ull,
+		                        0x963877195940eabdull, 0x96283ee2a88effe3ull, 0xbe5e1e2553863992ull,
+		                        0x2b0199fc2c85b8aaull, 0x0eb72ddc81c52ca2ull };
+		return v[i];
+	}
+	static __device__ __forceinline__ void compress(uint64_t st[8], uint64_t w[16]) { sha512_compress(st, w); }
+	// key word i: the digest's bytes 8i..8i+8 in order
+	static __device__ __forceinline__ uint64_t key_word(const uint64_t st[8], int i)
+	{
+		return sha_be64(make_uint2((uint32_t)st[i], (uint32_t)(st[i] >> 32)));
+	}
+};
+
+// The same arguments as k_block_sha256's
 __global__ void __launch_bounds__(SHA512_THREADS)
 k_block_sha512(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs,
     const uint8_t *__restrict__ d_out, const mtz_rec *__restrict__ orecs, uint32_t n, uint32_t mode,
     uint64_t base, BlockResult *__restrict__ res, const mtz_job *__restrict__ fjobs = nullptr,
     uint32_t frames = 0u)
 {
-	const uint32_t r = blockIdx.x * SHA512_THREADS + threadIdx.x;
-	if (r >= n) return;
-	const mtz_rec rec = recs[r];
-	if (rec.type != DRR_WRITE_T) return;
-	const uint8_t *hdr = d_in + rec.off;
-	const BlockClass c = block_classify(hdr, rec, mode, orecs != nullptr, ZIO_CKSUM_SHA512, frames);
-	if (c.what == 0) return;
-	const uint8_t *p;
-	uint64_t nbytes;
-	bool ok = true;
-	if (c.src == 0) {
-		p = hdr + DRR_HDR;
-		nbytes = (uint64_t)rec.payload;
-	} else if (fjobs == nullptr) {
-		const mtz_rec o = orecs[r];
-		p = d_out + o.off + DRR_HDR;
-		nbytes = (uint64_t)o.payload;
-		// the stage's encoder stored the block raw where ZFS's stored a frame: not that encoder
-		if (c.what == 2 && o.comp != ZIO_LZ4) ok = false;
-	} else {
-		// VERIFY with MTZ_FLAG_BLOCK_FRAMES / _LZJB: the declared encoder's frame (kernels_frames.cuh)
-		const mtz_job j = fjobs[r];
-		p = reinterpret_cast<const uint8_t *>((uintptr_t)j.dst_off);
-		nbytes = (uint64_t)j.out_len;
-		if (j.out_len >= rec.lsize) ok = false;
-	}
-	const uint64_t cover = (c.what == 1) ? c.lsz : c.psz;
-	if (nbytes > cover) ok = false;
-	if (ok) {
-		uint64_t st[8] = SHA512_256_IV;
-		const uint64_t nblk = cover / 128ull + 1ull;
-		uint64_t cur[16], nxt[16];
-		sha512_message_block(p, nbytes, cover, 0, cur);
-		for (uint64_t k = 0; k < nblk; k++) {
-			if (k + 1ull < nblk) sha512_message_block(p, nbytes, cover, k + 1ull, nxt);
-			sha512_compress(st, cur);
-#pragma unroll
-			for (int i = 0; i < 16; i++) cur[i] = nxt[i];
-		}
-		const uint64_t *key = reinterpret_cast<const uint64_t *>(hdr + 56);
-#pragma unroll
-		for (int i = 0; i < 4; i++)
-			ok = ok && key[i] == sha_be64(make_uint2((uint32_t)st[i], (uint32_t)(st[i] >> 32)));
-	}
-	atomicAdd(&res->sha512, 1ull);
-	block_verdict(res, c.what, ok, base + r);
+	block_sha<Sha512H>(d_in, recs, d_out, orecs, n, mode, base, res, fjobs, frames);
 }
 
 } // namespace mtz

@@ -24,18 +24,22 @@ namespace mtz {
 // block-check verdicts not yet folded into the handle: those of deferred batches wait for
 // mtz_dev_finish*, where the stream verdict of the same records surfaces
 struct BlockPending {
-	BlockResult r;
+	BlockResult r{};
 	uint64_t obj = 0, off = 0;    // drr_object / drr_offset of record r.first_bad
 	uint8_t ctype = 0;            // ... and its drr_checksumtype
-	BlockPending() { clear(); }
-	void clear()
-	{
-		r.logical_ok = r.frame_ok = r.frame_miss = r.skipped = r.sha256 = r.sha512 = r.frames = r.lzjb = r.zle = 0;
-		r.first_bad = r.first_miss = ~0ull;
-		obj = off = 0;
-		ctype = 0;
-	}
+	BlockPending() { r.first_bad = r.first_frame_miss = ~0ull; }
+	void clear() { *this = BlockPending(); }
 };
+
+// The counters of `r` added to those of the same names in `d` (a BlockResult or mtz_block_stats),
+// and the first frame miss of both kept.
+template <class Dst> static void block_add(Dst &d, const BlockResult &r)
+{
+	d.logical_ok += r.logical_ok; d.frame_ok += r.frame_ok; d.frame_miss += r.frame_miss; d.skipped += r.skipped;
+	d.sha256 += r.sha256; d.sha512 += r.sha512;
+	d.frames_encoded += r.frames_encoded; d.lzjb_encoded += r.lzjb_encoded; d.zle_encoded += r.zle_encoded;
+	d.first_frame_miss = d.first_frame_miss < r.first_frame_miss ? d.first_frame_miss : r.first_frame_miss;
+}
 
 // device scratch of one codec batch (modes COMPRESS / DECOMPRESS / RECOMPRESS); in VERIFY with
 // MTZ_FLAG_BLOCK_FRAMES / _LZJB the encoders' jobs, scratch and frame sums of the block check (enc, d_enc,

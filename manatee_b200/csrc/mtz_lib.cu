@@ -583,7 +583,7 @@ static uint32_t block_hashed(const mtz_handle *h)
 static int32_t block_reset(mtz_handle *h, cudaStream_t st, BlockResult *bres)
 {
 	MTZ_CU(h, cudaMemsetAsync(bres, 0, offsetof(BlockResult, first_bad), st));
-	MTZ_CU(h, cudaMemsetAsync(&bres->first_bad, 0xff, 2 * sizeof(unsigned long long), st));
+	MTZ_CU(h, cudaMemsetAsync(&bres->first_bad, 0xff, sizeof(BlockResult) - offsetof(BlockResult, first_bad), st));
 	return MTZ_OK;
 }
 
@@ -599,7 +599,7 @@ static int32_t launch_block(mtz_handle *h, cudaStream_t st, const uint8_t *d_in,
 	if (nrec == 0) return MTZ_OK;
 	const bool sha = block_sha256_on(h), sha512 = block_sha512_on(h);
 	const unsigned grid = (unsigned)((nrec + BLK_THREADS - 1) / BLK_THREADS);
-	k_block_check<<<grid, BLK_THREADS, 0, st>>>(d_in, d_recs, isums, orecs, osums, (uint32_t)nrec,
+	k_block_check<<<grid, BLK_THREADS, 0, st>>>(d_in, d_recs, isums, orecs, osums, d_out, (uint32_t)nrec,
 	    h->cfg.mode, base, bres, block_hashed(h), fjobs, block_fcodecs(h));
 	MTZ_CU(h, cudaGetLastError());
 	if (sha) {
@@ -662,10 +662,7 @@ static int32_t launch_block_frames(mtz_handle *h, cudaStream_t st, CodecBufs &cb
 static int32_t block_take(mtz_handle *h, BlockPending &p, const BlockResult &r, const uint8_t *d_in,
     uint64_t off)
 {
-	p.r.logical_ok += r.logical_ok; p.r.frame_ok += r.frame_ok;
-	p.r.frame_miss += r.frame_miss; p.r.skipped += r.skipped; p.r.sha256 += r.sha256;
-	p.r.sha512 += r.sha512; p.r.frames += r.frames; p.r.lzjb += r.lzjb; p.r.zle += r.zle;
-	p.r.first_miss = std::min(p.r.first_miss, r.first_miss);
+	block_add(p.r, r);
 	if (r.first_bad < p.r.first_bad) {
 		uint64_t w[6];      // header bytes 8..55: drr_object, drr_offset, drr_checksumtype
 		MTZ_CU(h, cudaMemcpy(w, d_in + off + 8, sizeof w, cudaMemcpyDeviceToHost));
@@ -684,12 +681,7 @@ static int32_t block_fold(mtz_handle *h, BlockPending &p, uint64_t stream_bad)
 	p.clear();
 	{
 		std::lock_guard<std::mutex> g(h->stats_mu);
-		h->bstats.logical_ok += q.r.logical_ok; h->bstats.frame_ok += q.r.frame_ok;
-		h->bstats.frame_miss += q.r.frame_miss; h->bstats.skipped += q.r.skipped;
-		h->bstats.sha256 += q.r.sha256; h->bstats.sha512 += q.r.sha512;
-		h->bstats.frames_encoded += q.r.frames;
-		h->bstats.lzjb_encoded += q.r.lzjb; h->bstats.zle_encoded += q.r.zle;
-		h->bstats.first_frame_miss = std::min<uint64_t>(h->bstats.first_frame_miss, q.r.first_miss);
+		block_add(h->bstats, q.r);
 	}
 	if (q.r.first_bad == ~0ull || q.r.first_bad >= stream_bad) return MTZ_OK;
 	{
@@ -1555,6 +1547,21 @@ static int32_t harvest(mtz_handle *h, Slot &s)
 	return rc;
 }
 
+// The block check of slot s's batch as far as its input goes, `isums` = the input's sums: the
+// results reset, then VERIFY's frames and their check (launch_block_frames) or the check of the input
+// records.  The codec modes check their records after the output's sums (codec_launch_post).
+static int32_t launch_block_input(mtz_handle *h, Slot &s, const RecSums *isums)
+{
+	if (!block_on(h) || s.nrec == 0) return MTZ_OK;
+	int32_t rc = block_reset(h, s.st, s.d_bres);
+	if (rc == MTZ_OK && block_frames_on(h))
+		rc = launch_block_frames(h, s.st, s.cb, s.d_in, s.d_recs, isums, s.nrec, 0,
+		    all_compact_blocks(s.h_recs, s.nrec), s.first_rec, s.d_bres);
+	else if (rc == MTZ_OK && !is_codec_mode(h->cfg.mode))
+		rc = launch_block(h, s.st, s.d_in, s.d_recs, isums, nullptr, nullptr, nullptr, s.nrec, s.first_rec, s.d_bres);
+	return rc;
+}
+
 // Enqueue one batch: the bytes come from up to two host pieces (ring wrap),
 // s.h_recs[0..nrec) is already filled with batch-relative offsets.
 static int32_t submit_batch(mtz_handle *h, Slot &s, const uint8_t *p0, size_t n0,
@@ -1581,16 +1588,8 @@ static int32_t submit_batch(mtz_handle *h, Slot &s, const uint8_t *p0, size_t n0
 		    nrec ? bytes / nrec : 0);
 		if (rc != MTZ_OK) return rc;
 		// the block check needs no running checksum: it runs now, its verdict waits with the stream's
-		if (block_on(h) && nrec > 0) {
-			rc = block_reset(h, s.st, s.d_bres);
-			if (rc == MTZ_OK && block_frames_on(h))
-				rc = launch_block_frames(h, s.st, s.cb, s.d_in, s.d_recs, h->dv_sums + h->dv_nrec, nrec, 0,
-				    all_compact_blocks(s.h_recs, nrec), s.first_rec, s.d_bres);
-			else if (rc == MTZ_OK)
-				rc = launch_block(h, s.st, s.d_in, s.d_recs, h->dv_sums + h->dv_nrec, nullptr, nullptr, nullptr,
-				    nrec, s.first_rec, s.d_bres);
-			if (rc != MTZ_OK) return rc;
-		}
+		rc = launch_block_input(h, s, h->dv_sums + h->dv_nrec);
+		if (rc != MTZ_OK) return rc;
 		if (h->dv_nrec == 0) h->dv_first = s.first_rec;
 		h->dv_nrec += nrec; h->dv_in_bytes += bytes; h->dv_st = h->st;
 	} else if (h->cfg.mode != MTZ_MODE_PASSTHROUGH) {
@@ -1598,17 +1597,8 @@ static int32_t submit_batch(mtz_handle *h, Slot &s, const uint8_t *p0, size_t n0
 		rc = launch_k1(h, s.st, s.d_in, s.d_recs, nrec, s.d_sums, s.ev_k1a, s.ev_k1b,
 		    nrec ? bytes / nrec : 0);
 		if (rc != MTZ_OK) return rc;
-		if (block_on(h) && nrec > 0) {
-			// VERIFY checks the input here; the codec modes after the output's sums (codec_launch_post)
-			rc = block_reset(h, s.st, s.d_bres);
-			if (rc == MTZ_OK && block_frames_on(h))
-				rc = launch_block_frames(h, s.st, s.cb, s.d_in, s.d_recs, s.d_sums, nrec, 0,
-				    all_compact_blocks(s.h_recs, nrec), s.first_rec, s.d_bres);
-			else if (rc == MTZ_OK && !is_codec_mode(h->cfg.mode))
-				rc = launch_block(h, s.st, s.d_in, s.d_recs, s.d_sums, nullptr, nullptr, nullptr, nrec, s.first_rec,
-				    s.d_bres);
-			if (rc != MTZ_OK) return rc;
-		}
+		rc = launch_block_input(h, s, s.d_sums);
+		if (rc != MTZ_OK) return rc;
 		if (is_codec_mode(h->cfg.mode)) {
 			rc = codec_reset(h, s.st, s.cb);
 			if (rc != MTZ_OK) return rc;
