@@ -99,7 +99,23 @@ extern "C" {
                                   * frame_ok or frame_miss (counted, never an error) and the output bytes do
                                   * not change.  mtz_block_stats.lzjb_encoded / zle_encoded count the frames
                                   * encoded; with this flag and batch_bytes 0 VERIFY batches are 256 MiB.
-                                  * COMPRESS and DECOMPRESS accept the flag and do not change */
+                                  * COMPRESS and DECOMPRESS accept the flag and do not change without
+                                  * MTZ_FLAG_BLOCK_LOGICAL */
+
+#define MTZ_FLAG_BLOCK_LOGICAL 128u /* with MTZ_FLAG_BLOCK_CKSUM only (MTZ_EINVAL without it), with or without the
+                                  * other block flags.  COMPRESS / DECOMPRESS / RECOMPRESS also check keys from
+                                  * the logical bytes they hold (the raw input payload, or the decoder's
+                                  * output for a record that arrives LZ4), so that a transfer over the
+                                  * compressed wire counts what VERIFY counts on the raw stream.
+                                  * RECOMPRESS: a block stored raw on disk that arrives LZ4 must match its
+                                  * decoded bytes (MTZ_ECKSUM otherwise, as in DECOMPRESS).  With
+                                  * MTZ_FLAG_BLOCK_LZJB: a record with an lzjb / zle key that arrives raw, or
+                                  * LZ4 in DECOMPRESS / RECOMPRESS (COMPRESS decodes nothing), gets a frame from the stage's lzjb / zle encoder as in VERIFY
+                                  * (frame_ok or frame_miss; lzjb_encoded / zle_encoded).  DECOMPRESS: a
+                                  * record with an LZ4 key that arrives raw is the frame_miss COMPRESS
+                                  * counted for it at the sender.  The output bytes and mtz_stats do not
+                                  * change; mtz_block_stats.logical_checked counts these records.  VERIFY
+                                  * accepts the flag and does not change */
 
 typedef struct mtz_handle mtz_handle;
 
@@ -167,6 +183,8 @@ typedef struct mtz_block_stats {
 	                               frame_ok / frame_miss, and in sha256 / sha512 where those hashed it) */
 	uint64_t lzjb_encoded;      /* MTZ_FLAG_BLOCK_LZJB: lzjb frames encoded for the check (likewise) */
 	uint64_t zle_encoded;       /* MTZ_FLAG_BLOCK_LZJB: zle frames encoded for the check (likewise) */
+	uint64_t logical_checked;   /* MTZ_FLAG_BLOCK_LOGICAL: records compared thanks to that flag (also counted
+	                               in logical_ok / frame_ok / frame_miss, or the cause of the failure) */
 } mtz_block_stats;
 
 /* One DRR record as seen by the kernels (32 B, little endian). */

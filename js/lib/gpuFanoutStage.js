@@ -57,7 +57,8 @@ function GpuFanoutStage(options) {
             (options.blockSha256 ? 8 : 0) |        // gpu.blockSha256: MTZ_FLAG_BLOCK_SHA256
             (options.blockSha512 ? 16 : 0) |       // gpu.blockSha512: MTZ_FLAG_BLOCK_SHA512
             (options.blockFrames ? 32 : 0) |       // gpu.blockFrames: MTZ_FLAG_BLOCK_FRAMES
-            (options.blockLzjb ? 64 : 0)           // gpu.blockLzjb: MTZ_FLAG_BLOCK_LZJB
+            (options.blockLzjb ? 64 : 0) |         // gpu.blockLzjb: MTZ_FLAG_BLOCK_LZJB
+            (options.blockLogical ? 128 : 0)       // gpu.blockLogical: MTZ_FLAG_BLOCK_LOGICAL
     });
     this._blockChecksums = !!options.blockChecksums;
     this._peers = [];

@@ -24,6 +24,7 @@ var BLOCK_SHA256 = 8;       // MTZ_FLAG_BLOCK_SHA256 (with BLOCK_CKSUM only)
 var BLOCK_SHA512 = 16;      // MTZ_FLAG_BLOCK_SHA512 (with BLOCK_CKSUM only)
 var BLOCK_FRAMES = 32;      // MTZ_FLAG_BLOCK_FRAMES (with BLOCK_CKSUM only)
 var BLOCK_LZJB = 64;        // MTZ_FLAG_BLOCK_LZJB (with BLOCK_CKSUM only)
+var BLOCK_LOGICAL = 128;    // MTZ_FLAG_BLOCK_LOGICAL (with BLOCK_CKSUM only)
 
 function GpuSnapshotStage(options) {
     if (!(this instanceof GpuSnapshotStage)) {
@@ -44,7 +45,8 @@ function GpuSnapshotStage(options) {
             (options.blockSha256 ? BLOCK_SHA256 : 0) |       // gpu.blockSha256
             (options.blockSha512 ? BLOCK_SHA512 : 0) |       // gpu.blockSha512
             (options.blockFrames ? BLOCK_FRAMES : 0) |       // gpu.blockFrames
-            (options.blockLzjb ? BLOCK_LZJB : 0)             // gpu.blockLzjb
+            (options.blockLzjb ? BLOCK_LZJB : 0) |           // gpu.blockLzjb
+            (options.blockLogical ? BLOCK_LOGICAL : 0)       // gpu.blockLogical
     });
     this._blockChecksums = !!options.blockChecksums;
     this._pending = null;      // {chunk, off, cb} waiting for ring space

@@ -335,6 +335,7 @@ static napi_value BlockStats(napi_env env, napi_callback_info info)
 	PUT("framesEncoded", frames_encoded);
 	PUT("lzjbEncoded", lzjb_encoded);
 	PUT("zleEncoded", zle_encoded);
+	PUT("logicalChecked", logical_checked);
 #undef PUT
 	// ~0 (no miss) does not survive a double: -1 says "none"
 	napi_create_double(env, st.first_frame_miss == ~0ull ? -1.0 : (double)st.first_frame_miss, &v);

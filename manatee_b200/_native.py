@@ -22,6 +22,7 @@ FLAG_BLOCK_SHA256 = 8
 FLAG_BLOCK_SHA512 = 16
 FLAG_BLOCK_FRAMES = 32
 FLAG_BLOCK_LZJB = 64
+FLAG_BLOCK_LOGICAL = 128
 XCHG_FIRST, XCHG_LAST = 1, 2
 MODE_NAMES = {"verify": 0, "compress": 1, "decompress": 2, "recompress": 3, "passthrough": 4}
 
@@ -57,7 +58,8 @@ class BlockStats(C.Structure):
                 ("frame_ok", C.c_uint64), ("frame_miss", C.c_uint64), ("skipped", C.c_uint64),
                 ("first_frame_miss", C.c_uint64), ("sha256", C.c_uint64),
                 ("sha512", C.c_uint64), ("frames_encoded", C.c_uint64),
-                ("lzjb_encoded", C.c_uint64), ("zle_encoded", C.c_uint64)]
+                ("lzjb_encoded", C.c_uint64), ("zle_encoded", C.c_uint64),
+                ("logical_checked", C.c_uint64)]
 
     def as_dict(self):
         return {k: getattr(self, k) for k, _ in self._fields_[2:]}

@@ -28,6 +28,14 @@ namespace mtz {
 #define BLK_FR_LZ4     1u      // MTZ_FLAG_BLOCK_FRAMES: LZ4 frames (K3)
 #define BLK_FR_LZJB    2u      // MTZ_FLAG_BLOCK_LZJB: lzjb and zle frames, and in VERIFY and
                                // RECOMPRESS lzjb / zle records that arrive as their disk frame
+#define BLK_FR_LOGICAL 4u      // MTZ_FLAG_BLOCK_LOGICAL: the re-encoding modes check keys from the logical
+                               // bytes they hold (k_logical_plan, kernels_frames.cuh)
+// BlockClass.src: where the bytes a key is compared with are
+#define BLK_SRC_IN     0       // the input payload
+#define BLK_SRC_OUT    1       // the output payload of a re-encoding mode
+#define BLK_SRC_JOB    2       // the check's own job (kernels_frames.cuh): a frame the declared encoder made
+                               // for the check, or the logical bytes K2 decoded
+#define BLK_SRC_NONE   3       // none: a miss by rule
 
 // The counters carry their mtz_block_stats names.
 struct BlockResult {           // device, mirrored to pinned host; zeroed per batch
@@ -36,6 +44,7 @@ struct BlockResult {           // device, mirrored to pinned host; zeroed per ba
 	unsigned long long sha512;       // records compared by k_block_sha512 (kernels_sha512.cuh)
 	unsigned long long frames_encoded;   // LZ4 frames encoded for the check (k_frame_sums, kernels_frames.cuh)
 	unsigned long long lzjb_encoded, zle_encoded;   // lzjb / zle frames encoded for the check (likewise)
+	unsigned long long logical_checked;    // records compared thanks to MTZ_FLAG_BLOCK_LOGICAL
 	unsigned long long first_bad;          // stream index of the first logical mismatch, ~0 none
 	unsigned long long first_frame_miss;   // stream index of the first frame mismatch, ~0 none
 };
@@ -57,15 +66,22 @@ __host__ __device__ __forceinline__ Ck4 strip_head8(const Ck4 &whole, const Ck4 
 }
 
 // What a record's key lets the stage compare, decided from its header alone, for keys of type
-// `ctype`: `what` 0 skipped, 1 the logical block, 2 the disk frame; `src` 0 the input payload, 1 the
-// output payload, or in VERIFY the frame the declared encoder made of the input (kernels_frames.cuh).
+// `ctype`: `what` 0 skipped, 1 the logical block, 2 the disk frame; `src` BLK_SRC_*.
 // `have_out` = the output records of a re-encoding mode are at hand; `frames` = BLK_FR_* bits: with
 // BLK_FR_LZ4 (VERIFY with MTZ_FLAG_BLOCK_FRAMES) the encoder's LZ4 frames of the raw records are, with
 // BLK_FR_LZJB (MTZ_FLAG_BLOCK_LZJB) lzjb and zle keys are checked: against the input payload when
 // the record arrives as that frame (VERIFY, RECOMPRESS: passed through), in VERIFY against the
-// encoder's frame of a raw record.  Every key type that is checked goes through this one table.
+// encoder's frame of a raw record.  With BLK_FR_LOGICAL the re-encoding modes also use the logical
+// bytes they hold (the raw input payload, or in DECOMPRESS and RECOMPRESS K2's output for a record that
+// arrives LZ4; COMPRESS decodes nothing, so an LZ4 record it is handed stays skipped), rows marked
+// `logical`: a raw-on-disk key of an LZ4 record in RECOMPRESS is compared with them; with BLK_FR_LZJB
+// an lzjb / zle key with the declared encoder's frame of them, as VERIFY does; and in DECOMPRESS a raw
+// record with an LZ4 key is the miss COMPRESS counted for it at the sender (a raw record on the
+// lz4-stage-v1 wire is one that stage's encoder stored raw).  Every key type that is checked goes
+// through this one table.
 struct BlockClass {
 	int what, src;
+	bool logical;
 	uint64_t lsz, psz;
 };
 
@@ -76,20 +92,27 @@ __device__ __forceinline__ BlockClass block_classify(const uint8_t *hdr, const m
 	BlockClass c;
 	c.lsz = ((prop & 0xffffull) + 1ull) * 512ull;
 	c.psz = (((prop >> 16) & 0xffffull) + 1ull) * 512ull;
-	c.what = 0; c.src = 0;
+	c.what = 0; c.src = BLK_SRC_IN; c.logical = false;
 	const uint32_t dc = (uint32_t)((prop >> 32) & 0x7full);
 	const bool raw_in = rec.comp == 0u, lz4_in = rec.comp == ZIO_LZ4;
 	const bool encodes = mode == MTZ_MODE_COMPRESS || mode == MTZ_MODE_RECOMPRESS;
+	const bool decodes = mode == MTZ_MODE_DECOMPRESS || mode == MTZ_MODE_RECOMPRESS;
+	// the logical bytes of a record that arrives LZ4 exist only where K2 decodes it: not in COMPRESS
+	const bool logical = (frames & BLK_FR_LOGICAL) && (raw_in ? (encodes || decodes) : (lz4_in && decodes));
 	if (hdr[48] == ctype && prop != 0ull && !((prop >> 39) & 1ull) && c.lsz == rec.lsize) {
 		if ((dc == BLK_DC_INHERIT || dc == BLK_DC_OFF) && c.psz == c.lsz) {
-			if (raw_in) { c.what = 1; c.src = 0; }
-			else if (lz4_in && mode == MTZ_MODE_DECOMPRESS && have_out) { c.what = 1; c.src = 1; }
+			if (raw_in) { c.what = 1; c.src = BLK_SRC_IN; }
+			else if (lz4_in && mode == MTZ_MODE_DECOMPRESS && have_out) { c.what = 1; c.src = BLK_SRC_OUT; }
+			else if (lz4_in && mode == MTZ_MODE_RECOMPRESS && logical) { c.what = 1; c.src = BLK_SRC_JOB; c.logical = true; }
 		} else if (dc == BLK_DC_LZ4) {
-			if (lz4_in) { c.what = 2; c.src = 0; }
-			else if (raw_in && ((encodes && have_out) || ((frames & BLK_FR_LZ4) && mode == MTZ_MODE_VERIFY))) { c.what = 2; c.src = 1; }
+			if (lz4_in) { c.what = 2; c.src = BLK_SRC_IN; }
+			else if (raw_in && encodes && have_out) { c.what = 2; c.src = BLK_SRC_OUT; }
+			else if (raw_in && (frames & BLK_FR_LZ4) && mode == MTZ_MODE_VERIFY) { c.what = 2; c.src = BLK_SRC_JOB; }
+			else if (raw_in && mode == MTZ_MODE_DECOMPRESS && logical) { c.what = 2; c.src = BLK_SRC_NONE; c.logical = true; }
 		} else if ((frames & BLK_FR_LZJB) && (dc == BLK_DC_LZJB || dc == BLK_DC_ZLE)) {
-			if (rec.comp == dc && (mode == MTZ_MODE_VERIFY || mode == MTZ_MODE_RECOMPRESS)) { c.what = 2; c.src = 0; }
-			else if (raw_in && mode == MTZ_MODE_VERIFY) { c.what = 2; c.src = 1; }
+			if (rec.comp == dc && (mode == MTZ_MODE_VERIFY || mode == MTZ_MODE_RECOMPRESS)) { c.what = 2; c.src = BLK_SRC_IN; }
+			else if (raw_in && mode == MTZ_MODE_VERIFY) { c.what = 2; c.src = BLK_SRC_JOB; }
+			else if ((raw_in || lz4_in) && logical) { c.what = 2; c.src = BLK_SRC_JOB; c.logical = true; }
 		}
 	}
 	return c;
@@ -126,11 +149,12 @@ __device__ __forceinline__ BlockClass block_class(const uint8_t *hdr, const mtz_
 }
 
 // Record r's key of type `ctype` against the bytes block_classify picks: the input payload, output
-// record r (at `d_out` + its offset) or VERIFY's frame job r (`fjobs`, kernels_frames.cuh), `nbytes`
-// of them at `p`, zero-extended to `cover`.  The stage's encoder storing the block raw where ZFS's
+// record r (at `d_out` + its offset) or the check's job r (`fjobs`, kernels_frames.cuh), `nbytes`
+// of them at `p`, zero-extended to `cover`.  An encoder storing the block raw where ZFS's
 // stored a frame (not that encoder) and bytes longer than the key covers are mismatches;
 // `match(p, nbytes, cover, src)` compares the rest.  The verdict goes to `res` as stream record
-// `base + r`, after a bump of res->*counter (null: none).  False: a key this kernel does not check.
+// `base + r`, after a bump of res->*counter (null: none) and, for a row of MTZ_FLAG_BLOCK_LOGICAL, of
+// res->logical_checked.  False: a key this kernel does not check.
 template <class Match>
 __device__ __forceinline__ bool block_compare(const uint8_t *hdr, const mtz_rec &rec, uint32_t r, uint32_t mode,
     uint32_t ctype, uint32_t frames, const mtz_rec *orecs, const uint8_t *d_out, const mtz_job *fjobs,
@@ -138,27 +162,27 @@ __device__ __forceinline__ bool block_compare(const uint8_t *hdr, const mtz_rec 
 {
 	const BlockClass c = block_class(hdr, rec, mode, ctype, frames, orecs);
 	if (c.what == 0) return false;
-	const uint8_t *p;
-	uint64_t nbytes;
+	const uint8_t *p = hdr + DRR_HDR;
+	uint64_t nbytes = (uint64_t)rec.payload;
 	bool ok = true;
-	if (c.src == 0) {
-		p = hdr + DRR_HDR;
-		nbytes = (uint64_t)rec.payload;
-	} else if (fjobs == nullptr) {
+	if (c.src == BLK_SRC_OUT) {
 		const mtz_rec o = orecs[r];
 		p = d_out + o.off + DRR_HDR;
 		nbytes = (uint64_t)o.payload;
 		if (c.what == 2 && o.comp != ZIO_LZ4) ok = false;
-	} else {
+	} else if (c.src == BLK_SRC_JOB) {
 		const mtz_job j = fjobs[r];
 		p = reinterpret_cast<const uint8_t *>((uintptr_t)j.dst_off);
 		nbytes = (uint64_t)j.out_len;
-		if (j.out_len >= rec.lsize) ok = false;      // stored raw
+		if (c.what == 2 && j.out_len >= rec.lsize) ok = false;      // stored raw
+	} else if (c.src == BLK_SRC_NONE) {
+		ok = false;
 	}
 	const uint64_t cover = (c.what == 1) ? c.lsz : c.psz;
 	if (nbytes > cover) ok = false;
 	if (ok) ok = match(p, nbytes, cover, c.src);
 	if (counter != nullptr) atomicAdd(&(res->*counter), 1ull);
+	if (c.logical) atomicAdd(&res->logical_checked, 1ull);
 	block_verdict(res, c.what, ok, base + r);
 	return true;
 }
@@ -167,9 +191,9 @@ __device__ __forceinline__ bool block_compare(const uint8_t *hdr, const mtz_rec 
 // the output records and their payload sums in the re-encoding modes (null in VERIFY), `d_out` the
 // output batch the offsets of `orecs` refer to.  Record r is record `base + r` of the stream.
 // `hashed` as block_key_checked's: the keys of those types this stage can check are left to the
-// kernel that hashes them instead of being counted as skipped.  `fjobs` (VERIFY with
-// MTZ_FLAG_BLOCK_FRAMES or MTZ_FLAG_BLOCK_LZJB, else null): the frame jobs of kernels_frames.cuh,
-// whose frames stand in for the output records and whose sums are in `osums`.  `frames`:
+// kernel that hashes them instead of being counted as skipped.  `fjobs` / `fsums` (VERIFY with
+// MTZ_FLAG_BLOCK_FRAMES or MTZ_FLAG_BLOCK_LZJB, the re-encoding modes with MTZ_FLAG_BLOCK_LOGICAL, else
+// null): the check's jobs of kernels_frames.cuh and the sums of their bytes.  `frames`:
 // block_classify's BLK_FR_* bits.
 #define BLK_THREADS 128
 __global__ void __launch_bounds__(BLK_THREADS)
@@ -177,7 +201,7 @@ k_block_check(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs
     const RecSums *__restrict__ isums, const mtz_rec *__restrict__ orecs,
     const RecSums *__restrict__ osums, const uint8_t *__restrict__ d_out, uint32_t n, uint32_t mode,
     uint64_t base, BlockResult *__restrict__ res, uint32_t hashed, const mtz_job *__restrict__ fjobs = nullptr,
-    uint32_t frames = 0u)
+    const RecSums *__restrict__ fsums = nullptr, uint32_t frames = 0u)
 {
 	const uint32_t r = blockIdx.x * BLK_THREADS + threadIdx.x;
 	if (r >= n) return;
@@ -187,12 +211,12 @@ k_block_check(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs
 	const bool checked = block_compare(hdr, rec, r, mode, ZIO_CKSUM_FLETCHER4, frames, orecs, d_out, fjobs, res,
 	    base, nullptr, [&](const uint8_t *, uint64_t nbytes, uint64_t cover, int src) {
 		Ck4 sums;
-		if (src == 0) {
+		if (src == BLK_SRC_IN) {
 			const RecSums s = isums[r];
 			const Ck4 zero = { 0, 0, 0, 0 };
 			sums = strip_head8(s.body, fold_cksum_words(zero, s.emb), s.nbody - 8u);
 		} else {
-			sums = osums[r].body;
+			sums = (src == BLK_SRC_OUT ? osums : fsums)[r].body;
 		}
 		return ck_eq(shift_zeros(sums, (cover - nbytes) >> 2), load_ck(hdr + 56));
 	});

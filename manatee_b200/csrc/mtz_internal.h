@@ -38,12 +38,15 @@ template <class Dst> static void block_add(Dst &d, const BlockResult &r)
 	d.logical_ok += r.logical_ok; d.frame_ok += r.frame_ok; d.frame_miss += r.frame_miss; d.skipped += r.skipped;
 	d.sha256 += r.sha256; d.sha512 += r.sha512;
 	d.frames_encoded += r.frames_encoded; d.lzjb_encoded += r.lzjb_encoded; d.zle_encoded += r.zle_encoded;
+	d.logical_checked += r.logical_checked;
 	d.first_frame_miss = d.first_frame_miss < r.first_frame_miss ? d.first_frame_miss : r.first_frame_miss;
 }
 
 // device scratch of one codec batch (modes COMPRESS / DECOMPRESS / RECOMPRESS); in VERIFY with
 // MTZ_FLAG_BLOCK_FRAMES / _LZJB the encoders' jobs, scratch and frame sums of the block check (enc, d_enc,
-// osums, k3_skip)
+// osums, k3_skip); in the codec modes with MTZ_FLAG_BLOCK_LOGICAL the jobs, sums and encoder scratch of the
+// block check's own (chk, chk_sums, d_chk, chk_pos): enc, d_enc and osums are K3's, k_assemble's and the
+// output K1's there
 struct CodecBufs {
 	size_t rec_cap = 0, scratch_cap = 0;
 	CodecRec *cr = nullptr;
@@ -55,6 +58,10 @@ struct CodecBufs {
 	uint8_t *d_logical = nullptr, *d_enc = nullptr;
 	uint32_t *seq_n = nullptr, *cert = nullptr;         // RECOMPRESS certificate: K2's parse sizes, K3c's verdicts
 	uint32_t *k3_skip = nullptr;                        // VERIFY with BLOCK_FRAMES and BLOCK_LZJB: K3 leaves these jobs
+	mtz_job *chk = nullptr;                             // BLOCK_LOGICAL: k_logical_plan's jobs
+	RecSums *chk_sums = nullptr;                        // ... and the sums of their bytes
+	uint8_t *d_chk = nullptr;                           // ... with BLOCK_LZJB: the slots of the lzjb / zle frames
+	unsigned long long *chk_pos = nullptr;              // ... and the running slot offset
 	CodecResult *d_cres = nullptr, *h_cres = nullptr;   // h_: pinned
 	ScanResult *d_ores = nullptr, *h_ores = nullptr;    // output-chain result
 	uint64_t *d_outpos = nullptr;                       // running output offset (device)

@@ -310,6 +310,8 @@ int32_t mtz_open(const mtz_config *cfg, mtz_handle **out)
 		return fail(nullptr, MTZ_EINVAL, "BLOCK_FRAMES extends the block check: it needs BLOCK_CKSUM");
 	if ((full.flags & MTZ_FLAG_BLOCK_LZJB) && !(full.flags & MTZ_FLAG_BLOCK_CKSUM))
 		return fail(nullptr, MTZ_EINVAL, "BLOCK_LZJB extends the block check: it needs BLOCK_CKSUM");
+	if ((full.flags & MTZ_FLAG_BLOCK_LOGICAL) && !(full.flags & MTZ_FLAG_BLOCK_CKSUM))
+		return fail(nullptr, MTZ_EINVAL, "BLOCK_LOGICAL extends the block check: it needs BLOCK_CKSUM");
 	const cudaDeviceProp &prop = props[0];
 
 	mtz_handle *h = new (std::nothrow) mtz_handle();
@@ -568,12 +570,20 @@ static bool block_frames_on(const mtz_handle *h)
 	return (h->cfg.flags & (MTZ_FLAG_BLOCK_FRAMES | MTZ_FLAG_BLOCK_LZJB)) != 0 && h->cfg.mode == MTZ_MODE_VERIFY;
 }
 static bool block_lzjb_on(const mtz_handle *h) { return (h->cfg.flags & MTZ_FLAG_BLOCK_LZJB) != 0; }
+static bool is_codec_mode(uint32_t m);
+// COMPRESS / DECOMPRESS / RECOMPRESS with MTZ_FLAG_BLOCK_LOGICAL: the block check runs jobs over the
+// logical bytes (launch_block_logical); VERIFY accepts the flag and does not change
+static bool block_logical_on(const mtz_handle *h)
+{
+	return (h->cfg.flags & MTZ_FLAG_BLOCK_LOGICAL) != 0 && is_codec_mode(h->cfg.mode);
+}
 // block_classify's BLK_FR_* bits: LZ4 frames in VERIFY with MTZ_FLAG_BLOCK_FRAMES (the codec modes have
-// their own), lzjb / zle keys with MTZ_FLAG_BLOCK_LZJB (block_classify limits them to VERIFY and RECOMPRESS)
+// their own), lzjb / zle keys with MTZ_FLAG_BLOCK_LZJB (block_classify limits them to VERIFY and RECOMPRESS,
+// and to the rows of MTZ_FLAG_BLOCK_LOGICAL)
 static uint32_t block_fcodecs(const mtz_handle *h)
 {
 	return ((h->cfg.flags & MTZ_FLAG_BLOCK_FRAMES) && h->cfg.mode == MTZ_MODE_VERIFY ? BLK_FR_LZ4 : 0u) |
-	    (block_lzjb_on(h) ? BLK_FR_LZJB : 0u);
+	    (block_lzjb_on(h) ? BLK_FR_LZJB : 0u) | (block_logical_on(h) ? BLK_FR_LOGICAL : 0u);
 }
 static uint32_t block_hashed(const mtz_handle *h)
 {
@@ -590,17 +600,18 @@ static int32_t block_reset(mtz_handle *h, cudaStream_t st, BlockResult *bres)
 // k_block_check over records [0, nrec) of a (sub-)batch, record 0 being stream record `base`, then
 // with MTZ_FLAG_BLOCK_SHA256 k_block_sha256 and with MTZ_FLAG_BLOCK_SHA512 k_block_sha512 over the
 // same records (`d_out` = the output batch the offsets of `orecs` refer to; null with `orecs`).
-// `fjobs`: VERIFY's frames (launch_block_frames), with their sums in `osums`.  Not counted in
-// mtz_stats.kernel_launches: the flags leave every mtz_stats field as it is.
+// `fjobs` / `fsums`: the check's own jobs and the sums of their bytes (launch_block_frames,
+// launch_block_logical).  Not counted in mtz_stats.kernel_launches: the flags leave every mtz_stats
+// field as it is.
 static int32_t launch_block(mtz_handle *h, cudaStream_t st, const uint8_t *d_in, const mtz_rec *d_recs,
     const RecSums *isums, const mtz_rec *orecs, const RecSums *osums, const uint8_t *d_out, size_t nrec,
-    uint64_t base, BlockResult *bres, const mtz_job *fjobs = nullptr)
+    uint64_t base, BlockResult *bres, const mtz_job *fjobs = nullptr, const RecSums *fsums = nullptr)
 {
 	if (nrec == 0) return MTZ_OK;
 	const bool sha = block_sha256_on(h), sha512 = block_sha512_on(h);
 	const unsigned grid = (unsigned)((nrec + BLK_THREADS - 1) / BLK_THREADS);
 	k_block_check<<<grid, BLK_THREADS, 0, st>>>(d_in, d_recs, isums, orecs, osums, d_out, (uint32_t)nrec,
-	    h->cfg.mode, base, bres, block_hashed(h), fjobs, block_fcodecs(h));
+	    h->cfg.mode, base, bres, block_hashed(h), fjobs, fsums, block_fcodecs(h));
 	MTZ_CU(h, cudaGetLastError());
 	if (sha) {
 		const unsigned gs = (unsigned)((nrec + SHA_THREADS - 1) / SHA_THREADS);
@@ -653,7 +664,33 @@ static int32_t launch_block_frames(mtz_handle *h, cudaStream_t st, CodecBufs &cb
 	const unsigned gs = (unsigned)std::min<size_t>((nrec + K1_WARPS - 1) / K1_WARPS, (size_t)h->sm_count * 16);
 	k_frame_sums<<<gs, K1_THREADS, 0, st>>>(cb.enc, n, cb.osums, bres);
 	MTZ_CU(h, cudaGetLastError());
-	return launch_block(h, st, d_in, d_recs, isums, nullptr, cb.osums, nullptr, nrec, base, bres, cb.enc);
+	return launch_block(h, st, d_in, d_recs, isums, nullptr, nullptr, nullptr, nrec, base, bres, cb.enc, cb.osums);
+}
+
+// The jobs of the block check of a codec (sub-)batch with MTZ_FLAG_BLOCK_LOGICAL, into cb.chk /
+// cb.chk_sums (kernels_frames.cuh): plan, with MTZ_FLAG_BLOCK_LZJB the lzjb and zle encoders into cb.d_chk,
+// and the sums of the frames and of the logical bytes of the identity jobs.  It reads the input
+// batch, K2's jobs and cb.d_logical, so it runs where codec_launch_post does, after k_assemble has
+// read the same; like the rest of the check, nothing here is counted in mtz_stats.
+static int32_t launch_block_logical(mtz_handle *h, cudaStream_t st, CodecBufs &cb, const uint8_t *d_in,
+    const mtz_rec *d_recs, size_t nrec, BlockResult *bres)
+{
+	const uint32_t n = (uint32_t)nrec;
+	if (cb.d_chk != nullptr) MTZ_CU(h, cudaMemsetAsync(cb.chk_pos, 0, sizeof(unsigned long long), st));
+	k_logical_plan<<<(n + FRP_THREADS - 1) / FRP_THREADS, FRP_THREADS, 0, st>>>(d_in, d_recs, n, h->cfg.mode,
+	    block_hashed(h), block_fcodecs(h), cb.dec, cb.d_chk, cb.chk_pos, cb.chk);
+	MTZ_CU(h, cudaGetLastError());
+	if (cb.d_chk != nullptr) {
+		const unsigned gl = (unsigned)std::min<size_t>((nrec + LZJB_WARPS - 1) / LZJB_WARPS, (size_t)h->sm_count * 8);
+		k_lzjb_encode<<<gl, LZJB_THREADS, 0, st>>>(cb.chk, n);
+		MTZ_CU(h, cudaGetLastError());
+		k_zle_encode<<<gl, LZJB_THREADS, 0, st>>>(cb.chk, n);
+		MTZ_CU(h, cudaGetLastError());
+	}
+	const unsigned gs = (unsigned)std::min<size_t>((nrec + K1_WARPS - 1) / K1_WARPS, (size_t)h->sm_count * 16);
+	k_frame_sums<<<gs, K1_THREADS, 0, st>>>(cb.chk, n, cb.chk_sums, bres);
+	MTZ_CU(h, cudaGetLastError());
+	return MTZ_OK;
 }
 
 // Merge a batch's results (host copy) into `p`; on a mismatch read drr_object / drr_offset of the
@@ -747,6 +784,14 @@ static int32_t codec_alloc(mtz_handle *h, CodecBufs &cb, size_t rec_cap, size_t 
 	if (h->cfg.mode != MTZ_MODE_DECOMPRESS) MTZ_CU(h, cudaMalloc(&cb.d_enc, scratch_cap + 512));
 	if (h->cfg.mode == MTZ_MODE_VERIFY && block_lzjb_on(h) && (h->cfg.flags & MTZ_FLAG_BLOCK_FRAMES))
 		MTZ_CU(h, cudaMalloc(&cb.k3_skip, rec_cap * sizeof(uint32_t)));
+	if (block_logical_on(h)) {
+		MTZ_CU(h, cudaMalloc(&cb.chk, rec_cap * sizeof(mtz_job)));
+		MTZ_CU(h, cudaMalloc(&cb.chk_sums, rec_cap * sizeof(RecSums)));
+		if (block_lzjb_on(h)) {
+			MTZ_CU(h, cudaMalloc(&cb.d_chk, scratch_cap + 512));
+			MTZ_CU(h, cudaMalloc(&cb.chk_pos, sizeof(unsigned long long)));
+		}
+	}
 	if (certify_on(h)) {
 		MTZ_CU(h, cudaMalloc(&cb.seq_n, rec_cap * sizeof(uint32_t)));
 		MTZ_CU(h, cudaMalloc(&cb.cert, rec_cap * sizeof(uint32_t)));
@@ -766,6 +811,7 @@ static void codec_free(CodecBufs &cb)
 	cudaFree(cb.dec); cudaFree(cb.enc); cudaFree(cb.out_recs); cudaFree(cb.osums); cudaFree(cb.steps);
 	cudaFree(cb.d_logical); cudaFree(cb.d_enc); cudaFree(cb.d_cres); cudaFree(cb.d_ores);
 	cudaFree(cb.d_outpos); cudaFree(cb.seq_n); cudaFree(cb.cert); cudaFree(cb.k3_skip);
+	cudaFree(cb.chk); cudaFree(cb.chk_sums); cudaFree(cb.d_chk); cudaFree(cb.chk_pos);
 	if (cb.h_cres) cudaFreeHost(cb.h_cres);
 	if (cb.h_ores) cudaFreeHost(cb.h_ores);
 	cb = CodecBufs();
@@ -878,7 +924,9 @@ static int32_t codec_launch_post(mtz_handle *h, cudaStream_t st, CodecBufs &cb, 
 	// output records of a codec batch are smaller than the logical size: decide by the input's
 	launch_k1_kernel(h, st, d_out, orecs, n, osums, 312u, cb.avg_out_rec);
 	if (bres != nullptr) {
-		const int32_t rc = launch_block(h, st, d_in, d_recs, isums, orecs, osums, d_out, nrec, bbase, bres);
+		int32_t rc = block_logical_on(h) ? launch_block_logical(h, st, cb, d_in, d_recs, nrec, bres) : MTZ_OK;
+		if (rc == MTZ_OK)
+			rc = launch_block(h, st, d_in, d_recs, isums, orecs, osums, d_out, nrec, bbase, bres, cb.chk, cb.chk_sums);
 		if (rc != MTZ_OK) return rc;
 	}
 	if (all_osums == nullptr) {

@@ -135,7 +135,8 @@ class BackupSender(object):
                                 block_sha256=bool(g.get("blockSha256")),
                                 block_sha512=bool(g.get("blockSha512")),
                                 block_frames=bool(g.get("blockFrames")),
-                                block_lzjb=bool(g.get("blockLzjb")))
+                                block_lzjb=bool(g.get("blockLzjb")),
+                                block_logical=bool(g.get("blockLogical")))
 
     def _stage_stats(self, stage):
         """job.gpu: the stage counters, plus `blocks` (block-checksum counters) with

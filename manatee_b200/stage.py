@@ -21,7 +21,7 @@ class GpuSnapshotStage(object):
 
     def __init__(self, mode="verify", device=0, ring_bytes=0, batch_bytes=0, n_slots=0,
                  out_ring_bytes=0, flags=0, devices=None, block_checksums=False, block_sha256=False,
-                 block_sha512=False, block_frames=False, block_lzjb=False):
+                 block_sha512=False, block_frames=False, block_lzjb=False, block_logical=False):
         """``devices`` = CUDA ordinals of a device group: the GPUs of one box run as ONE stage,
         batch b of the stream on ``devices[b % len(devices)]`` (mtz_config.devices[]).
         ``block_checksums`` = MTZ_FLAG_BLOCK_CKSUM: every DRR_WRITE is also checked against the
@@ -37,7 +37,14 @@ class GpuSnapshotStage(object):
         ``block_lzjb`` = MTZ_FLAG_BLOCK_LZJB: keys over an lzjb or zle frame on disk are checked too:
         a record that arrives as that frame (VERIFY, RECOMPRESS) as it is, a raw one in VERIFY
         against the stage's lzjb / zle encoder frame of it (``block_stats()["lzjb_encoded"]``,
-        ``["zle_encoded"]``).  With or without ``block_frames``; only valid with ``block_checksums``."""
+        ``["zle_encoded"]``).  With or without ``block_frames``; only valid with ``block_checksums``.
+        ``block_logical`` = MTZ_FLAG_BLOCK_LOGICAL: COMPRESS, DECOMPRESS and RECOMPRESS also check keys
+        from the logical bytes they hold, so that a transfer over the compressed wire counts what
+        VERIFY counts on the raw stream: RECOMPRESS compares a raw-on-disk key of an LZ4 record with
+        the decoded bytes (ECKSUM on a mismatch), with ``block_lzjb`` the three modes encode lzjb / zle
+        frames of raw and LZ4 records as VERIFY does, and DECOMPRESS counts a raw record with an LZ4
+        key as the frame miss the sender counted (``block_stats()["logical_checked"]``).  VERIFY
+        accepts it and does not change.  Only valid with ``block_checksums``."""
         if block_checksums:
             flags |= N.FLAG_BLOCK_CKSUM
         if block_sha256:
@@ -48,6 +55,8 @@ class GpuSnapshotStage(object):
             flags |= N.FLAG_BLOCK_FRAMES
         if block_lzjb:
             flags |= N.FLAG_BLOCK_LZJB
+        if block_logical:
+            flags |= N.FLAG_BLOCK_LOGICAL
         self._L = N.lib()
         self._h = C.c_void_p()
         cfg = N.Config()

@@ -63,8 +63,9 @@ def lz4_keyed(O, s, threads):
     return s
 
 
-def kernel_times(fn, n):
-    """device ms per step of the frame kernels (torch.profiler, CUDA activities), over n steps"""
+def kernel_times(fn, n, kernels=None):
+    """device ms per step of `kernels` (default KERNELS, the frame kernels; torch.profiler, CUDA
+    activities), over n steps"""
     import torch
     from torch.profiler import ProfilerActivity, profile
     torch.cuda.synchronize()
@@ -73,7 +74,7 @@ def kernel_times(fn, n):
             fn()
         torch.cuda.synchronize()
     res = {}
-    for kern in KERNELS:
+    for kern in kernels or KERNELS:
         us, calls = 0.0, 0
         for e in prof.key_averages():
             if kern in e.key:

@@ -43,11 +43,16 @@ PARAMS = {
                                                             (131072, 9, True)],
     "test_sha256_and_sha512_keys": [("sha256",), ("sha512",)],
     "test_send_c_stream_frames_checked_as_they_arrive": [("verify",), ("recompress",)],
+    "test_the_compressed_wire_counts_what_verify_counts": [(dict(sha256=False, sha512=False, lzjb=False),),
+                                                           (dict(sha256=True, sha512=True, lzjb=True),)],
+    "test_a_corrupted_raw_keyed_lz4_record_fails_the_recompress_relay": [("fletcher4",), ("sha256",), ("sha512",)],
 }
 SKIP = {"test_sixteen_mib_record": "16 MiB blocks take minutes per encode on the emulator",
         "test_size_independent_properties_at_2gib": "2 GiB of LZ4 work is out of reach for the emulator",
         "test_device_api_across_the_subbatch_edge": "66 000 records; tests/test_emul_block_cksum.py crosses the "
                                                     "emulated build's 700-record edge instead",
+        "test_deferred_codec_shards": "its device buffers are torch tensors; tests/test_emul_block_logical.py runs it "
+                                      "on host memory",
         "test_device_group": "needs two GPUs",
         "test_real_streams_with_lzjb_or_zle_keys": "tests/golden/real holds no stream with lzjb or zle keys"}
 
@@ -67,12 +72,13 @@ def main():
     import test_gpu_block_sha512 as W
     import test_gpu_block_frames as F
     import test_gpu_block_lzjb as J
+    import test_gpu_block_logical as L
     import test_gpu_codec as K
     import test_gpu_lz4 as Z
     import test_gpu_stream as S
     import test_gpu_verify as V
     tot = fail = 0
-    for mod in (V, S, Z, K, B, H, W, F, J):
+    for mod in (V, S, Z, K, B, H, W, F, J, L):
         for name, fn in inspect.getmembers(mod, inspect.isfunction):
             if not name.startswith("test_") or filt not in name:
                 continue
