@@ -1,6 +1,6 @@
 /* lzjb_zfs.c -- TEST INFRASTRUCTURE: ZFS's lzjb and zle encoders and decoders, restated in C
  * ([EXTERNAL] lzjb.c, zle.c), driven the way zio_compress_data drives them.  Built and loaded by
- * tests/block_lzjb_ref.py (compiled into a temporary directory on first use); the GPU encoders of
+ * tests/lzjb_ref.py (compiled into a temporary directory on first use); the GPU encoders of
  * manatee_b200/csrc/kernels_lzjb.cuh are held to it.
  *
  * lzjb's table keeps the low 16 bits of source POINTERS, so its output depends on the address of

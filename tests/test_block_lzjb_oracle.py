@@ -1,12 +1,14 @@
-"""CPU: the lzjb / zle restatements and the model of MTZ_FLAG_BLOCK_LZJB (tests/block_lzjb_ref.py).
-The pure-Python encoders equal ZFS's C code (tests/lzjb_zfs.c) on fuzzed and edge inputs, every
-frame decodes to its input in both languages, a few answers are derived by hand, lzjb's dependence on
-the buffer's address phase is shown, and the model with the flag off (or on streams without lzjb / zle
-keys) is the existing one."""
+"""CPU: the lzjb / zle restatements (tests/lzjb_ref.py) and the model of MTZ_FLAG_BLOCK_LZJB
+(tests/block_ref.py).  The pure-Python encoders equal ZFS's C code (tests/lzjb_zfs.c) on fuzzed and
+edge inputs, every frame decodes to its input in both languages, a few answers are derived by hand,
+lzjb's dependence on the buffer's address phase is shown, and turning the flag off skips exactly the
+lzjb / zle keys (none on streams without them) and changes no other verdict."""
 import numpy as np
 import pytest
 
-import block_lzjb_ref as R
+import block_ref as R
+import lzjb_ref as Z
+import test_block_cksum_oracle as T
 import test_gpu_block_lzjb as G
 
 SIZES = [512, 1024, 4096, 8192, 65536, 131072, 1 << 20]
@@ -24,18 +26,18 @@ def _payloads(oracle, size, seed):
 
 def _both(x):
     """(python, C) results of both encoders for x: the c_len and frame of each"""
-    pl, cl = R.py_lzjb_compress(x), R.zfs_lzjb_compress(x)
-    pz, cz = R.py_zle_compress(x), R.zfs_zle_compress(x)
+    pl, cl = Z.py_lzjb_compress(x), Z.zfs_lzjb_compress(x)
+    pz, cz = Z.py_zle_compress(x), Z.zfs_zle_compress(x)
     return (pl, cl), (pz, cz)
 
 
 def _check(x):
     n = len(x)
     for (py, (zio, c_len)), dec_py, dec_c in (
-            (_both(x)[0], R.py_lzjb_decompress, R.zfs_lzjb_decompress),
-            (_both(x)[1], R.py_zle_decompress, R.zfs_zle_decompress)):
+            (_both(x)[0], Z.py_lzjb_decompress, Z.zfs_lzjb_decompress),
+            (_both(x)[1], Z.py_zle_decompress, Z.zfs_zle_decompress)):
         assert py[0] == c_len
-        assert R.zio_rule(py[0], py[1], n) == zio
+        assert Z.zio_rule(py[0], py[1], n) == zio
         if py[1] is not None:
             assert zio[1] is None or zio[1][:len(py[1])] == py[1]
             assert dec_py(py[1], n) == x and dec_c(py[1], n) == x
@@ -68,8 +70,8 @@ def test_lzjb_gives_up_exactly_at_the_copymap_test():
     for n in (512, 520, 1024, 4096):
         for pre in range(0, 200, 7):
             x = bytes(pre) + rng.integers(0, 256, n - pre, dtype=np.uint8).tobytes()
-            py = R.py_lzjb_compress(x)
-            assert py[0] == R.zfs_lzjb_compress(x)[1]
+            py = Z.py_lzjb_compress(x)
+            assert py[0] == Z.zfs_lzjb_compress(x)[1]
             seen.add(py[0] == n)
     assert seen == {True, False}
 
@@ -115,17 +117,17 @@ def test_known_answers():
     (252, 1), at offset 66 (252, 66).
     zle, 1024 zero bytes: five runs of 192 (length byte 192 - 1 + 64 = 255) and one of 64 (127):
     6 bytes, padded to 512 < 1024, so ZFS stores the frame."""
-    c_len, fr = R.py_lzjb_compress(b"\x01" * 1024)
+    c_len, fr = Z.py_lzjb_compress(b"\x01" * 1024)
     assert c_len == 71 and fr[:8] == bytes([0xfe, 1, 252, 1, 252, 66, 252, 66])
     assert fr[-2:] == b"\x00\x01" and fr[-11:-2] == b"\x00" + b"\x01" * 8      # items 40..47
-    assert R.zfs_lzjb_compress(b"\x01" * 1024)[1] == 71
-    assert R.py_zle_compress(bytes(1024)) == (6, bytes([255] * 5 + [127]))
-    assert R.zfs_zle_compress(bytes(1024))[0] == (512, bytes([255] * 5 + [127]) + bytes(506))
+    assert Z.zfs_lzjb_compress(b"\x01" * 1024)[1] == 71
+    assert Z.py_zle_compress(bytes(1024)) == (6, bytes([255] * 5 + [127]))
+    assert Z.zfs_zle_compress(bytes(1024))[0] == (512, bytes([255] * 5 + [127]) + bytes(506))
     # 512 zero bytes: 3 bytes, but the pad reaches LSIZE: stored raw
-    assert R.zfs_zle_compress(bytes(512))[0] == (512, None)
+    assert Z.zfs_zle_compress(bytes(512))[0] == (512, None)
     # random bytes: every encoder gives up, the block is stored raw
     x = np.random.default_rng(0).integers(0, 256, 8192, dtype=np.uint8).tobytes()
-    assert R.py_lzjb_compress(x)[0] == R.py_zle_compress(x)[0] == 8192
+    assert Z.py_lzjb_compress(x)[0] == Z.py_zle_compress(x)[0] == 8192
 
 
 def _phase_block(seed):
@@ -148,13 +150,13 @@ def test_lzjb_depends_on_the_buffer_phase():
     differ = 0
     for seed in range(64):
         x = _phase_block(seed)
-        (_, f0), c0 = R.zfs_lzjb_compress(x, 0)
-        (_, f5), c5 = R.zfs_lzjb_compress(x, 512)
-        py = R.py_lzjb_compress(x)
+        (_, f0), c0 = Z.zfs_lzjb_compress(x, 0)
+        (_, f5), c5 = Z.zfs_lzjb_compress(x, 512)
+        py = Z.py_lzjb_compress(x)
         assert py[0] == c0 and (f0 is None or f0[:c0] == py[1])
         if f0 is not None and f5 is not None and f0 != f5:
             differ += 1
-            assert R.zfs_lzjb_decompress(f0, len(x)) == x == R.zfs_lzjb_decompress(f5, len(x))
+            assert Z.zfs_lzjb_decompress(f0, len(x)) == x == Z.zfs_lzjb_decompress(f5, len(x))
     assert differ > 0
 
 
@@ -162,40 +164,36 @@ def test_most_data_does_not_depend_on_the_phase(oracle):
     same = 0
     for seed in range(20):
         x = oracle.gen_payload(oracle.PAYLOAD_PGPAGE, seed, 131072).tobytes()
-        same += R.zfs_lzjb_compress(x, 0) == R.zfs_lzjb_compress(x, 512)
+        same += Z.zfs_lzjb_compress(x, 0) == Z.zfs_lzjb_compress(x, 512)
     assert same >= 18
 
 
 def test_the_model_with_the_flag_off_is_the_existing_one(oracle):
-    s, _ = G._mixed(oracle)
+    s, dcs = G._mixed(oracle)
+    c = R.as_send_c(oracle, s)
+    ncomp = sum(1 for x in dcs.values() if x in (R.DC_LZJB, R.DC_ZLE))
     for frames in (False, True):
-        v, st = R.block_check_lzjb(oracle, s, frames=frames, lzjb=False)
-        if frames:
-            v0, st0 = R.block_check_frames(oracle, s)
-        else:
-            v0, st0 = R.block_check(s, None, R.VERIFY)
-        assert v == v0 and all(st[k] == st0[k] for k in st0)
-        assert st["lzjb_encoded"] == st["zle_encoded"] == 0
+        assert T.flag_off(oracle, s, R.VERIFY, None, "lzjb", frames=frames) == ncomp
+        assert T.flag_off(oracle, c, R.VERIFY, None, "lzjb", frames=frames) == ncomp
+    assert T.flag_off(oracle, c, R.RECOMPRESS, oracle.stream_recompress(c)[1], "lzjb") == ncomp
 
 
 def test_the_model_without_lzjb_or_zle_keys_is_the_existing_one(oracle):
     from test_gpu_codec import _mixed_stream
-    s, _ = R.as_lz4_on_disk(oracle, _mixed_stream(oracle, n=20, recsize=8192))
+    s, _ = R.as_on_disk(oracle, _mixed_stream(oracle, n=20, recsize=8192))
     for frames in (False, True):
-        on = R.block_check_lzjb(oracle, s, frames=frames)
-        off = R.block_check_lzjb(oracle, s, frames=frames, lzjb=False)
-        assert on == off
+        assert T.flag_off(oracle, s, R.VERIFY, None, "lzjb", frames=frames) == 0
 
 
 def test_the_model_checks_every_lzjb_and_zle_key(oracle):
     s, dcs = G._mixed(oracle)
-    v, st = R.block_check_lzjb(oracle, s)
+    v, st = R.block_check(oracle, s, R.VERIFY, lzjb=True)
     nl = sum(1 for x in dcs.values() if x == R.DC_LZJB)
     nz = sum(1 for x in dcs.values() if x == R.DC_ZLE)
     assert nl > 0 and nz > 0 and st["lzjb_encoded"] == nl and st["zle_encoded"] == nz
     assert st["frame_ok"] == nl + nz and st["frame_miss"] == 0
     # the send -c form: the same frames arrive as they are, nothing is encoded
     c = R.as_send_c(oracle, s)
-    _, sc = R.block_check_lzjb(oracle, c)
+    _, sc = R.block_check(oracle, c, R.VERIFY, lzjb=True)
     assert sc["frame_ok"] == st["frame_ok"] + sum(1 for x in dcs.values() if x == R.DC_LZ4)
     assert sc["lzjb_encoded"] == sc["zle_encoded"] == 0

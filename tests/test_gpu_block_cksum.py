@@ -1,6 +1,8 @@
 """GPU: MTZ_FLAG_BLOCK_CKSUM through the C ABI -- every DRR_WRITE checked against the on-disk block
 checksum its header carries (drr_key), on process_host, the ring API, the device API (sub-batched
-and deferred) and a device group, against the reference model in tests/block_cksum_ref.py.
+and deferred) and a device group, against the reference model in tests/block_ref.py.  The stage helpers here
+(_stage, _run, _want, _same, _fails) take the model's flags (sha256=, sha512=, frames=, lzjb=,
+logical=) and are those of every test_gpu_block_*.py; _same compares every counter the library reports.
 
 A block stored raw on disk must equal its logical bytes: a stream that was corrupted and then
 re-stamped passes every stream checksum and fails here.  A block stored LZ4 on disk is compared with
@@ -10,33 +12,57 @@ import threading
 import numpy as np
 import pytest
 
-import block_cksum_ref as R
+import block_ref as R
 
 pytestmark = pytest.mark.gpu
 
 MODES = {"verify": R.VERIFY, "compress": R.COMPRESS, "decompress": R.DECOMPRESS, "recompress": R.RECOMPRESS}
 TIMING = ("gpu_ms", "k1_ms", "codec_ms", "k3_ms")
-COUNTERS = ("logical_ok", "frame_ok", "frame_miss", "skipped", "first_frame_miss")
+FLAGS = ("sha256", "sha512", "frames", "lzjb", "logical")
 
 
-def _run(oracle, mode, s, flag=True, **kw):
-    """process_host -> (output, stats, block stats); the output of VERIFY is the input"""
+def _stage(mode, cksum=True, **kw):
+    """a stage with block_checksums = `cksum`; the model's flags in `kw` become its block_* arguments"""
     from manatee_b200 import GpuSnapshotStage
+    for f in FLAGS:
+        if f in kw:
+            kw["block_" + f] = kw.pop(f)
+    return GpuSnapshotStage(mode, block_checksums=cksum, **kw)
+
+
+def _run(oracle, mode, s, **kw):
+    """process_host -> (output, stats without the timing fields, block stats); the output of VERIFY is
+    the input.  `kw` as _stage's."""
     out = None if mode == "verify" else np.zeros(s.size * 3 + (1 << 20), dtype=np.uint8)
-    with GpuSnapshotStage(mode, block_checksums=flag, **kw) as g:
+    with _stage(mode, **kw) as g:
         n = g.process_host(s, out)
-        return (s if out is None else out[:n].copy()), g.stats(), g.block_stats()
+        st = g.stats()
+        for k in TIMING:
+            st.pop(k)
+        return (s if out is None else out[:n].copy()), st, g.block_stats()
 
 
-def _want(oracle, mode, inp, out):
-    """reference counters for a run of `mode` on `inp` that produced `out` (wire form)"""
+def _want(oracle, mode, inp, out, **flags):
+    """the model's verdicts and counters for a run of `mode` on `inp` that produced `out` (wire form)"""
     plain_in = oracle.wire_strip(inp) if mode == "decompress" else inp
     plain_out = None if mode == "verify" else oracle.wire_strip(out)
-    return R.block_check(plain_in, plain_out, MODES[mode])
+    return R.block_check(oracle, plain_in, MODES[mode], plain_out, **flags)
 
 
 def _same(bs, want):
-    assert {k: bs[k] for k in COUNTERS} == {k: want[k] for k in COUNTERS}, (bs, want)
+    assert {k: bs[k] for k in R.COUNTERS} == {k: want[k] for k in R.COUNTERS}, (bs, want)
+
+
+def _fails(mode, src, rec, **kw):
+    """the stage fails `src` with ECKSUM at record `rec`; returns the message.  `kw` as _stage's."""
+    from manatee_b200._native import MtzError, ECKSUM
+    out = np.zeros(src.size * 4 + (1 << 20), dtype=np.uint8)
+    with _stage(mode, **kw) as g:
+        with pytest.raises(MtzError) as ei:
+            g.process_host(src, None if mode == "verify" else out)
+        assert ei.value.code == ECKSUM, mode
+        assert g.stats()["bad_record"] == rec, mode
+        return str(ei.value)
 
 
 def _raw_stream(oracle, n=24, recsize=8192):
@@ -46,7 +72,7 @@ def _raw_stream(oracle, n=24, recsize=8192):
 
 def _mixed(oracle, n=30, recsize=8192, ashift=9):
     from test_gpu_codec import _mixed_stream
-    return R.as_lz4_on_disk(oracle, _mixed_stream(oracle, n=n, recsize=recsize), ashift)
+    return R.as_on_disk(oracle, _mixed_stream(oracle, n=n, recsize=recsize), ashift)
 
 
 def _corrupt_restamped(oracle, s, k, byte=1234):
@@ -77,37 +103,23 @@ def test_raw_stream_every_block_matches_in_every_mode(oracle):
 def test_corrupted_then_restamped_block_fails_only_with_the_flag(oracle):
     """The case the check exists for: the stream checksums are all valid, the bytes are not the
     primary's.  Reported at the reference's record, with the object and offset, in every mode."""
-    from manatee_b200._native import MtzError, ECKSUM
     s = _corrupt_restamped(oracle, oracle.synth_stream(40, recsize=16384, kind=oracle.PAYLOAD_PGPAGE), 17)
-    _, want = R.block_check(s, None, R.VERIFY)
+    _, want = R.block_check(oracle, s, R.VERIFY)
     assert want["first_bad"] == 17
-    _run(oracle, "verify", s, flag=False)
-    c, _, _ = _run(oracle, "compress", s, flag=False)
+    _run(oracle, "verify", s, cksum=False)
+    c, _, _ = _run(oracle, "compress", s, cksum=False)
     for mode, src in (("verify", s), ("compress", s), ("recompress", s), ("decompress", c)):
-        from manatee_b200 import GpuSnapshotStage
-        out = np.zeros(s.size * 3 + (1 << 20), dtype=np.uint8)
-        with GpuSnapshotStage(mode, block_checksums=True, batch_bytes=1 << 18) as g:
-            with pytest.raises(MtzError) as ei:
-                g.process_host(src, None if mode == "verify" else out)
-            assert ei.value.code == ECKSUM, mode
-            assert g.stats()["bad_record"] == 17, mode
-            msg = str(ei.value)
-            assert "block checksum" in msg and "object 8" in msg and "offset %d" % (15 * 16384) in msg, msg
+        msg = _fails(mode, src, 17, batch_bytes=1 << 18)
+        assert "block checksum" in msg and "object 8" in msg and "offset %d" % (15 * 16384) in msg, msg
 
 
 def test_flipped_key_bit_fails(oracle):
-    from manatee_b200._native import MtzError, ECKSUM
     s = _raw_stream(oracle).copy()
     _, offs = oracle.stream_index(s)
     s[int(offs[9]) + 56 + 17] ^= 0x40
     assert oracle.stream_restamp(s)[0] == 0
-    _run(oracle, "verify", s, flag=False)
-    from manatee_b200 import GpuSnapshotStage
-    with GpuSnapshotStage("verify", block_checksums=True) as g:
-        with pytest.raises(MtzError) as ei:
-            g.process_host(s)
-        assert ei.value.code == ECKSUM and "block checksum" in str(ei.value)
-        assert g.stats()["bad_record"] == 9
+    _run(oracle, "verify", s, cksum=False)
+    assert "block checksum" in _fails("verify", s, 9)
 
 
 @pytest.mark.parametrize("ashift,recsize", [(9, 8192), (12, 8192), (12, 65536)])
@@ -137,7 +149,7 @@ def test_frame_miss_is_counted_not_an_error(oracle):
         R.set_key(s, int(offs[i]), key=key, ddk_prop=(p & ~0xffff) | (R.get_key(s, int(offs[i]))[2] & 0xffff))
     assert oracle.stream_restamp(s)[0] == 0
     for mode in ("compress", "recompress"):
-        ref, _, _ = _run(oracle, mode, s, flag=False)
+        ref, _, _ = _run(oracle, mode, s, cksum=False)
         out, _, bs = _run(oracle, mode, s)
         assert np.array_equal(out, ref)
         _, want = _want(oracle, mode, s, out)
@@ -151,7 +163,7 @@ def test_send_c_stream_frames_checked_on_input(oracle, ashift):
     c = R.as_send_c(oracle, s, ashift)
     assert oracle.stream_verify(c)[0] == 0
     for mode in ("verify", "recompress"):
-        ref, _, _ = _run(oracle, mode, c, flag=False)
+        ref, _, _ = _run(oracle, mode, c, cksum=False)
         out, _, bs = _run(oracle, mode, c)
         assert np.array_equal(out, ref)
         _, want = _want(oracle, mode, c, out)
@@ -169,23 +181,21 @@ def test_unverifiable_keys_are_skipped(oracle):
     R.set_key(s, o[3], ddk_prop=0)
     assert oracle.stream_restamp(s)[0] == 0
     _, _, bs = _run(oracle, "verify", s)
-    _, want = R.block_check(s, None, R.VERIFY)
+    _, want = R.block_check(oracle, s, R.VERIFY)
     assert want["skipped"] == 4 and want["logical_ok"] == 8
     _same(bs, want)
 
 
 def test_passthrough_with_the_flag_is_einval(oracle):
-    from manatee_b200 import GpuSnapshotStage
     from manatee_b200._native import MtzError, EINVAL
     with pytest.raises(MtzError) as ei:
-        GpuSnapshotStage("passthrough", block_checksums=True)
+        _stage("passthrough")
     assert ei.value.code == EINVAL
 
 
 def test_first_failing_record_in_stream_order_is_reported(oracle):
     """One batch holds a block failure and a stream failure: the earlier record is reported; a record
     failing both reports its stream checksum."""
-    from manatee_b200 import GpuSnapshotStage
     from manatee_b200._native import MtzError, ECKSUM
     base = oracle.synth_stream(20, recsize=8192, kind=oracle.PAYLOAD_PGPAGE)
     _, offs = oracle.stream_index(base)
@@ -201,7 +211,7 @@ def test_first_failing_record_in_stream_order_is_reported(oracle):
     cases.append((s, 7, "stream checksum"))
     for s, rec, what in cases:
         assert oracle.stream_verify(s)[1].bad_record == rec or what == "block checksum"
-        with GpuSnapshotStage("verify", block_checksums=True) as g:
+        with _stage("verify") as g:
             with pytest.raises(MtzError) as ei:
                 g.process_host(s)
             assert ei.value.code == ECKSUM and what in str(ei.value), (rec, str(ei.value))
@@ -210,17 +220,15 @@ def test_first_failing_record_in_stream_order_is_reported(oracle):
 
 def test_the_flag_changes_no_byte_and_no_stats_field(oracle):
     s, _ = _mixed(oracle)
-    c, _, _ = _run(oracle, "compress", s, flag=False)
+    c, _, _ = _run(oracle, "compress", s, cksum=False)
     for mode, src in (("verify", s), ("compress", s), ("recompress", s), ("decompress", c),
                       ("recompress", R.as_send_c(oracle, s))):
-        a, sa, _ = _run(oracle, mode, src, flag=False, batch_bytes=1 << 18)
-        b, sb, bs = _run(oracle, mode, src, flag=True, batch_bytes=1 << 18)
+        a, sa, _ = _run(oracle, mode, src, cksum=False, batch_bytes=1 << 18)
+        b, sb, bs = _run(oracle, mode, src, batch_bytes=1 << 18)
         assert np.array_equal(a, b), mode
-        for k in TIMING:
-            sa.pop(k); sb.pop(k)
         assert sa == sb, mode
         assert bs["logical_ok"] + bs["frame_ok"] > 0
-    _, _, off = _run(oracle, "verify", s, flag=False)
+    _, _, off = _run(oracle, "verify", s, cksum=False)
     assert all(v == 0 for v in off.values())
 
 
@@ -252,12 +260,11 @@ def _pump(stage, data, chunk):
 
 @pytest.mark.parametrize("chunk", [4093, 1 << 20])
 def test_ring_api(oracle, chunk):
-    from manatee_b200 import GpuSnapshotStage
     from manatee_b200._native import MtzError, ECKSUM
     s, _ = _mixed(oracle)
     c = R.as_send_c(oracle, s)
     for mode in ("verify", "recompress"):
-        with GpuSnapshotStage(mode, block_checksums=True, batch_bytes=1 << 18) as g:
+        with _stage(mode, batch_bytes=1 << 18) as g:
             out, err = _pump(g, c.tobytes(), chunk)
             assert not err, err
             _, want = _want(oracle, mode, c, np.frombuffer(out, dtype=np.uint8))
@@ -265,7 +272,7 @@ def test_ring_api(oracle, chunk):
     # a failing block: no byte of its batch reaches the consumer
     bad = _corrupt_restamped(oracle, _raw_stream(oracle, n=40), 20)
     _, offs = oracle.stream_index(bad)
-    with GpuSnapshotStage("verify", block_checksums=True, batch_bytes=1 << 16) as g:
+    with _stage("verify", batch_bytes=1 << 16) as g:
         out, err = _pump(g, bad.tobytes(), chunk)
         assert any(isinstance(e, MtzError) and e.code == ECKSUM for e in err), err
         assert len(out) <= int(offs[20]) and g.stats()["bad_record"] == 20
@@ -291,7 +298,7 @@ class TorchMem(object):
 def device_api_subbatched(oracle, mem, nrec):
     """DECOMPRESS on the device API over more records than one codec sub-batch holds: records that
     arrive LZ4 are checked on the decoded output, the ones stored raw on the input."""
-    from manatee_b200 import GpuSnapshotStage, index_host
+    from manatee_b200 import index_host
     s = oracle.synth_stream(nrec, recsize=4096, kind=oracle.PAYLOAD_PGPAGE)
     rc, c, _ = oracle.stream_compress_plain(s)
     assert rc == 0
@@ -300,11 +307,11 @@ def device_api_subbatched(oracle, mem, nrec):
     d_recs, p_recs = mem.put(recs.view(np.uint8))
     cap = s.size + (1 << 20)
     d_out, p_out = mem.zeros(cap)
-    with GpuSnapshotStage("decompress", block_checksums=True) as g:
+    with _stage("decompress") as g:
         g.dev_submit(p_in, c.size, p_recs, len(recs), p_out, cap)
         ob, _, _ = g.dev_finish()
         out = mem.get(d_out, ob)
-        _, want = R.block_check(c, out, R.DECOMPRESS)
+        _, want = R.block_check(oracle, c, R.DECOMPRESS, out)
         assert want["logical_ok"] == nrec
         _same(g.block_stats(), want)
     from manatee_b200._native import MtzError, ECKSUM
@@ -313,7 +320,7 @@ def device_api_subbatched(oracle, mem, nrec):
     rb, _ = index_host(cb)
     d_in2, p_in2 = mem.put(cb)
     d_r2, p_r2 = mem.put(rb.view(np.uint8))
-    with GpuSnapshotStage("decompress", block_checksums=True) as g:
+    with _stage("decompress") as g:
         g.dev_submit(p_in2, cb.size, p_r2, len(rb), p_out, cap)
         with pytest.raises(MtzError) as ei:
             g.dev_finish()
@@ -327,14 +334,14 @@ def test_device_api_across_the_subbatch_edge(oracle):
 def test_deferred_shards(oracle):
     """MTZ_FLAG_DEFER_VERIFY: the block verdict of a shard surfaces at mtz_dev_finish, with the
     stream verdict, at the stream-wide record index."""
-    from manatee_b200 import GpuSnapshotStage, index_host
+    from manatee_b200 import index_host
     from manatee_b200._native import FLAG_DEFER_VERIFY, MtzError, ECKSUM
     s = oracle.synth_stream(60, recsize=16384, kind=oracle.PAYLOAD_PGPAGE)
     recs, _ = index_host(s)
     cut = int(recs["off"][31])
     for bad_rec, fails in ((None, None), (40, 1), (12, 0)):
         src = s if bad_rec is None else _corrupt_restamped(oracle, s, bad_rec)
-        gs = [GpuSnapshotStage("verify", batch_bytes=1 << 18, flags=FLAG_DEFER_VERIFY, block_checksums=True)
+        gs = [_stage("verify", batch_bytes=1 << 18, flags=FLAG_DEFER_VERIFY)
               for _ in range(2)]
         try:
             gs[0].process_host(src[:cut]); gs[1].process_host(src[cut:])

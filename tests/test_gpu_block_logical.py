@@ -5,14 +5,14 @@ COMPRESS on it, in DECOMPRESS on the COMPRESS output and in RECOMPRESS on its co
 every subset of the SHA and lzjb flags.  A raw-keyed record corrupted inside its LZ4 frame fails a
 RECOMPRESS relay with the flag and travels on without it.  Covered on process_host, the ring API and
 the device API (sub-batched and deferred shards).  Every counter is the reference model's
-(tests/block_logical_ref.py); the output bytes and the non-timing mtz_stats fields are those of the
+(tests/block_ref.py); the output bytes and the non-timing mtz_stats fields are those of the
 flag off."""
 import itertools
 
 import numpy as np
 import pytest
 
-import block_logical_ref as R
+import block_ref as R
 import test_gpu_block_cksum as B
 
 pytestmark = pytest.mark.gpu
@@ -20,27 +20,12 @@ pytestmark = pytest.mark.gpu
 MODES = ("compress", "decompress", "recompress")
 SUBSETS = [dict(zip(("sha256", "sha512", "lzjb"), v)) for v in itertools.product((False, True), repeat=3)]
 ALL = dict(sha256=True, sha512=True, lzjb=True)
+ON = dict(frames=True, logical=True, **ALL)         # every flag: the stage of the invariant
+OFF = dict(frames=True, **ALL)                      # the same without MTZ_FLAG_BLOCK_LOGICAL
 
 
-def _kw(flags, logical):
-    return dict(block_checksums=True, block_frames=True, block_sha256=flags["sha256"], block_sha512=flags["sha512"],
-                block_lzjb=flags["lzjb"], block_logical=logical)
-
-
-def _run(mode, s, flags=ALL, logical=True, **kw):
-    """process_host -> (output, stats without the timing fields, block stats)"""
-    from manatee_b200 import GpuSnapshotStage
-    out = None if mode == "verify" else np.zeros(s.size * 3 + (1 << 20), dtype=np.uint8)
-    with GpuSnapshotStage(mode, **_kw(flags, logical), **kw) as g:
-        n = g.process_host(s, out)
-        st = g.stats()
-        for k in B.TIMING:
-            st.pop(k)
-        return (s if out is None else out[:n].copy()), st, g.block_stats()
-
-
-def _same(bs, want, keys=R.COUNTERS):
-    assert {k: bs[k] for k in keys} == {k: want[k] for k in keys}, (bs, want)
+def _same_as_verify(bs, v):
+    assert {k: bs[k] for k in R.TRANSFER} == {k: v[k] for k in R.TRANSFER}, (bs, v)
 
 
 def _inputs(oracle, x):
@@ -55,16 +40,16 @@ def _inputs(oracle, x):
 def test_the_compressed_wire_counts_what_verify_counts(oracle, flags):
     x, dcs = R.mixed_keys_stream(oracle, n=48)
     want = R.four_ways(oracle, x, frames=True, **flags)
-    _, _, v = _run("verify", x, flags, logical=False)
-    _same(v, want["verify"][1])
+    _, _, v = B._run(oracle, "verify", x, frames=True, **flags)
+    B._same(v, want["verify"][1])
     assert v["skipped"] < len(dcs) and (not flags["lzjb"] or v["lzjb_encoded"] > 0 < v["zle_encoded"])
     for mode, src in _inputs(oracle, x).items():
         for kw in (dict(batch_bytes=1 << 18), {})[:2 if flags == ALL else 1]:
-            a, sa, ba = _run(mode, src, flags, logical=False, **kw)
-            b, sb, bb = _run(mode, src, flags, **kw)
+            a, sa, ba = B._run(oracle, mode, src, frames=True, **flags, **kw)
+            b, sb, bb = B._run(oracle, mode, src, frames=True, logical=True, **flags, **kw)
             assert np.array_equal(a, b) and sa == sb, mode
-            _same(bb, want[mode][1], R.COUNTERS + ("logical_checked",))
-            _same(bb, v)
+            B._same(bb, want[mode][1])
+            _same_as_verify(bb, v)
             assert ba["logical_checked"] == 0 and bb["frames_encoded"] == 0
             assert bb["logical_checked"] == ba["skipped"] - bb["skipped"], (mode, ba, bb)
         assert bb["logical_checked"] > 0 or mode != "recompress" and not flags["lzjb"], (mode, bb)
@@ -73,19 +58,16 @@ def test_the_compressed_wire_counts_what_verify_counts(oracle, flags):
 def test_without_the_flag_the_modes_count_what_they_did(oracle):
     x, _ = R.mixed_keys_stream(oracle, n=30)
     for mode, src in _inputs(oracle, x).items():
-        out, _, bs = _run(mode, src, logical=False)
-        plain = oracle.wire_strip(src) if mode == "decompress" else src
-        _, want = R.block_check_lzjb(oracle, plain, mode=B.MODES[mode], lzjb=True, sha256=True, sha512=True,
-                                     out=oracle.wire_strip(out))
-        _same(bs, want)
+        out, _, bs = B._run(oracle, mode, src, **OFF)
+        B._same(bs, B._want(oracle, mode, src, out, **OFF)[1])
         assert bs["logical_checked"] == 0
 
 
 def test_verify_accepts_the_flag_and_does_not_change(oracle):
     x, _ = R.mixed_keys_stream(oracle, n=30)
     for src in (x, R.send_c_form(oracle, x)):
-        a, sa, ba = _run("verify", src, logical=False)
-        b, sb, bb = _run("verify", src)
+        a, sa, ba = B._run(oracle, "verify", src, **OFF)
+        b, sb, bb = B._run(oracle, "verify", src, **ON)
         assert np.array_equal(a, b) and sa == sb and ba == bb and bb["logical_checked"] == 0
 
 
@@ -122,51 +104,44 @@ def _corrupt_a_literal(oracle, c, k):
 def test_a_corrupted_raw_keyed_lz4_record_fails_the_recompress_relay(oracle, name):
     """a compression=off dataset on the compressed wire: the relay's decoder output is not the block on
     disk, the stream checksums (re-stamped) all hold"""
-    from manatee_b200 import GpuSnapshotStage
-    from manatee_b200._native import MtzError, ECKSUM
     x = oracle.synth_stream(40, recsize=16384, kind=oracle.PAYLOAD_PGPAGE)
     if name != "fletcher4":
         x = R.as_sha(oracle, x, name)
     bad = _corrupt_a_literal(oracle, R.send_c_form(oracle, x), 17)
-    _, want = R.block_check_logical(oracle, bad, R.RECOMPRESS, oracle.stream_recompress(bad)[1], sha256=True, sha512=True)
+    _, want = R.block_check(oracle, bad, R.RECOMPRESS, oracle.stream_recompress(bad)[1], sha256=True, sha512=True,
+                            logical=True)
     assert want["first_bad"] == 17
-    _, _, off = _run("recompress", bad, logical=False)
+    _, _, off = B._run(oracle, "recompress", bad, **OFF)
     assert off["logical_ok"] == 0 and off["skipped"] == 40
     for kw in (dict(batch_bytes=1 << 18), {}):
-        out = np.zeros(x.size * 2, dtype=np.uint8)
-        with GpuSnapshotStage("recompress", **_kw(ALL, True), **kw) as g:
-            with pytest.raises(MtzError) as ei:
-                g.process_host(bad, out)
-            msg = str(ei.value)
-            assert ei.value.code == ECKSUM and g.stats()["bad_record"] == 17
-            assert "block checksum" in msg and "object 8" in msg and "offset %d" % (15 * 16384) in msg, msg
-            assert ("(%s key)" % name in msg) == (name != "fletcher4"), msg
+        msg = B._fails("recompress", bad, 17, **ON, **kw)
+        assert "block checksum" in msg and "object 8" in msg and "offset %d" % (15 * 16384) in msg, msg
+        assert ("(%s key)" % name in msg) == (name != "fletcher4"), msg
 
 
 @pytest.mark.parametrize("chunk", [4093, 1 << 20])
 def test_ring_api(oracle, chunk):
-    from manatee_b200 import GpuSnapshotStage
     x, _ = R.mixed_keys_stream(oracle, n=40)
     want = R.four_ways(oracle, x, frames=True, **ALL)
     for mode, src in _inputs(oracle, x).items():
         for kw in (dict(batch_bytes=1 << 18), {}):
-            with GpuSnapshotStage(mode, **_kw(ALL, True), **kw) as g:
+            with B._stage(mode, **ON, **kw) as g:
                 out, err = B._pump(g, src.tobytes(), chunk)
                 assert not err, err
-                assert out == _run(mode, src, logical=False)[0].tobytes()
-                _same(g.block_stats(), want[mode][1], R.COUNTERS + ("logical_checked",))
+                assert out == B._run(oracle, mode, src, **OFF)[0].tobytes()
+                B._same(g.block_stats(), want[mode][1])
 
 
 def _dev_run(mem, mode, src, recs=None, logical=True, flags=0, finish=True):
     """one device-API submit of the plain stream `src` -> (stage, device output, its capacity)"""
-    from manatee_b200 import GpuSnapshotStage, index_host
+    from manatee_b200 import index_host
     if recs is None:
         recs, _ = index_host(src)
     d_in, p_in = mem.put(src)
     d_recs, p_recs = mem.put(recs.view(np.uint8))
     cap = int(recs["lsize"].sum()) + int(src.size) + (1 << 20)
     d_out, p_out = mem.zeros(cap)
-    g = GpuSnapshotStage(mode, flags=flags, **_kw(ALL, logical))
+    g = B._stage(mode, flags=flags, **(ON if logical else OFF))
     g.dev_submit(p_in, src.size, p_recs, len(recs), p_out, cap)
     g._keep = (d_in, d_recs, d_out)
     return g, d_out
@@ -193,8 +168,8 @@ def compress_of_lz4_records(oracle, mem):
             ob, _, _ = g.dev_finish()
             got.append((mem.get(d_out, ob), g.block_stats()))
     assert np.array_equal(got[0][0], got[1][0]) and got[0][1] == got[1][1]
-    _, want = R.block_check_logical(oracle, c, R.COMPRESS, got[1][0], frames=True, **ALL)
-    _same(got[1][1], want, R.COUNTERS + ("logical_checked",))
+    _, want = R.block_check(oracle, c, R.COMPRESS, got[1][0], **ON)
+    B._same(got[1][1], want)
     assert want["skipped"] == 12 and want["logical_checked"] == 0
 
 
@@ -219,7 +194,7 @@ def device_api_subbatched(oracle, mem, nrec, modes=MODES, recsize=4096):
                 ob, _, _ = g.dev_finish()
                 outs.append(mem.get(d_out, ob))
                 if logical:
-                    _same(g.block_stats(), want[mode][1], R.COUNTERS + ("logical_checked",))
+                    B._same(g.block_stats(), want[mode][1])
         assert np.array_equal(outs[0], outs[1]), mode
     if "recompress" not in modes:
         return
@@ -248,7 +223,7 @@ def deferred_shards(oracle, mem):
     late = [i for i in raw_lz4 if i > cut][0]
     for bad in (None, late):
         src = c if bad is None else _corrupt_a_literal(oracle, c, bad)
-        _, want = R.block_check_logical(oracle, src, R.RECOMPRESS, oracle.stream_recompress(src)[1], frames=True, **ALL)
+        _, want = R.block_check(oracle, src, R.RECOMPRESS, oracle.stream_recompress(src)[1], **ON)
         recs, _ = index_host(src)
         cut_off = int(recs["off"][cut])
         parts = [(src[:cut_off], recs[:cut].copy()), (src[cut_off:], recs[cut:].copy())]
@@ -260,7 +235,7 @@ def deferred_shards(oracle, mem):
             if bad is None:
                 gs[1].dev_finish(carry_in=SH.carry_before(1, aggs), carry_out_in=co)
                 b0, b1 = gs[0].block_stats(), gs[1].block_stats()
-                for k in R.COUNTERS + ("logical_checked",):
+                for k in R.COUNTERS:
                     if k != "first_frame_miss":
                         assert b0[k] + b1[k] == want[k], (k, b0, b1, want)
             else:
@@ -283,5 +258,5 @@ def test_device_group(oracle):
     x, _ = R.mixed_keys_stream(oracle, n=40)
     want = R.four_ways(oracle, x, frames=True, **ALL)
     for mode, src in _inputs(oracle, x).items():
-        _, _, bs = _run(mode, src, devices=[0, 1], batch_bytes=1 << 18)
-        _same(bs, want[mode][1])
+        _, _, bs = B._run(oracle, mode, src, devices=[0, 1], batch_bytes=1 << 18, **ON)
+        B._same(bs, want[mode][1])

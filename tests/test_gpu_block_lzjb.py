@@ -3,7 +3,7 @@ frame.  In VERIFY a block that arrives raw is encoded by the declared encoders (
 k_zle_encode) beside the batch and compared as the LZ4 frames of MTZ_FLAG_BLOCK_FRAMES are; a block
 that arrives as its frame (`send -c`) is compared as it is, in VERIFY and RECOMPRESS.  Covered on
 process_host, the ring API, the device API (sub-batched and deferred) and a device group.  Every
-counter is the reference model's (tests/block_lzjb_ref.py); the output bytes and the non-timing
+counter is the reference model's (tests/block_ref.py); the output bytes and the non-timing
 mtz_stats fields are those of the flag off."""
 import glob
 import os
@@ -11,29 +11,10 @@ import os
 import numpy as np
 import pytest
 
-import block_lzjb_ref as R
+import block_ref as R
 import test_gpu_block_cksum as B
 
 pytestmark = pytest.mark.gpu
-
-COUNTERS = B.COUNTERS + ("sha256", "sha512", "frames_encoded", "lzjb_encoded", "zle_encoded")
-
-
-def _stage(mode, lzjb=True, frames=False, **kw):
-    from manatee_b200 import GpuSnapshotStage
-    return GpuSnapshotStage(mode, block_checksums=True, block_lzjb=lzjb, block_frames=frames, **kw)
-
-
-def _run(oracle, mode, s, lzjb=True, frames=False, **kw):
-    """process_host -> (output, stats, block stats); the output of VERIFY is the input"""
-    out = None if mode == "verify" else np.zeros(s.size * 3 + (1 << 20), dtype=np.uint8)
-    with _stage(mode, lzjb, frames, **kw) as g:
-        n = g.process_host(s, out)
-        return (s if out is None else out[:n].copy()), g.stats(), g.block_stats()
-
-
-def _same(bs, want, keys=COUNTERS):
-    assert {k: bs[k] for k in keys} == {k: want[k] for k in keys}, (bs, want)
 
 
 def _mixed(oracle, n=30, recsize=8192, ashift=9, codec=R.mixed_codecs):
@@ -49,10 +30,10 @@ def _count(dcs, dc):
 
 def _verify_matches_model(oracle, s, dcs, frames=False, sha256=False, sha512=False, **kw):
     """VERIFY + lzjb on `s`: the model's counters; every lzjb / zle key is frame_ok"""
-    kw.update(block_sha256=sha256, block_sha512=sha512)
-    _, st, bs = _run(oracle, "verify", s, frames=frames, **kw)
-    _, want = R.block_check_lzjb(oracle, s, frames=frames, sha256=sha256, sha512=sha512)
-    _same(bs, want)
+    flags = dict(lzjb=True, frames=frames, sha256=sha256, sha512=sha512)
+    _, st, bs = B._run(oracle, "verify", s, **flags, **kw)
+    _, want = R.block_check(oracle, s, R.VERIFY, **flags)
+    B._same(bs, want)
     assert bs["lzjb_encoded"] == _count(dcs, R.DC_LZJB) and bs["zle_encoded"] == _count(dcs, R.DC_ZLE)
     assert bs["frames_encoded"] == (_count(dcs, R.DC_LZ4) if frames else 0)
     assert bs["frame_miss"] == 0 and st["bad_record"] == R.NONE
@@ -82,11 +63,9 @@ def test_sixteen_mib_record(oracle):
 def test_the_output_and_the_stats_are_those_of_the_flag_off(oracle):
     s, dcs = _mixed(oracle)
     for kw in (dict(batch_bytes=1 << 18), {}):
-        a, sa, ba = _run(oracle, "verify", s, lzjb=False, **kw)
-        b, sb, bb = _run(oracle, "verify", s, **kw)
+        a, sa, ba = B._run(oracle, "verify", s, **kw)
+        b, sb, bb = B._run(oracle, "verify", s, lzjb=True, **kw)
         assert np.array_equal(a, b)
-        for k in B.TIMING:
-            sa.pop(k); sb.pop(k)
         assert sa == sb
         assert ba["lzjb_encoded"] == ba["zle_encoded"] == 0
         assert bb["lzjb_encoded"] + bb["zle_encoded"] == ba["skipped"] - bb["skipped"] > 0
@@ -102,7 +81,7 @@ def test_the_flag_without_block_checksums_is_einval(oracle):
                 GpuSnapshotStage(mode, **kw)
             assert ei.value.code == EINVAL, (mode, kw)
     with pytest.raises(MtzError) as ei:
-        _stage("passthrough")
+        B._stage("passthrough", lzjb=True)
     assert ei.value.code == EINVAL
 
 
@@ -116,10 +95,10 @@ def test_swapped_keys_are_counted_not_errors(oracle):
         R.set_key(s, int(offs[i]), key=key, ddk_prop=(p & ~0xffff) | (R.get_key(s, int(offs[i]))[2] & 0xffff))
     assert oracle.stream_restamp(s)[0] == 0
     for frames in (False, True):
-        _, st, bs = _run(oracle, "verify", s, frames=frames)
-        _, want = R.block_check_lzjb(oracle, s, frames=frames)
+        _, st, bs = B._run(oracle, "verify", s, frames=frames, lzjb=True)
+        _, want = R.block_check(oracle, s, R.VERIFY, lzjb=True, frames=frames)
         assert want["frame_miss"] == 3 and want["first_frame_miss"] == comp[1]
-        _same(bs, want)
+        B._same(bs, want)
         assert st["bad_record"] == R.NONE
 
 
@@ -130,10 +109,10 @@ def test_corrupted_then_restamped_records(oracle):
         idx = sorted(i for i, v in dcs.items() if v == dc)
         k = idx[len(idx) // 2]
         c = B._corrupt_restamped(oracle, s, k, byte=100)
-        _, st, bs = _run(oracle, "verify", c, batch_bytes=1 << 18)
-        _, want = R.block_check_lzjb(oracle, c)
+        _, st, bs = B._run(oracle, "verify", c, batch_bytes=1 << 18, lzjb=True)
+        _, want = R.block_check(oracle, c, R.VERIFY, lzjb=True)
         assert want["frame_miss"] == 1 and want["first_frame_miss"] == k
-        _same(bs, want)
+        B._same(bs, want)
         assert st["bad_record"] == R.NONE
 
 
@@ -145,7 +124,7 @@ def test_sha256_and_sha512_keys(oracle, name):
         bs = _verify_matches_model(oracle, src, dcs, frames=frames, **{name: True})
         assert bs[name] == len(dcs) - (0 if frames else _count(dcs, R.DC_LZ4))
     # without the hash's flag the records stay skipped: nothing is encoded for them
-    _, _, off = _run(oracle, "verify", src)
+    _, _, off = B._run(oracle, "verify", src, lzjb=True)
     assert off["lzjb_encoded"] == off["zle_encoded"] == 0 and off["skipped"] == len(dcs)
 
 
@@ -153,42 +132,36 @@ def test_sha256_and_sha512_keys(oracle, name):
 def test_send_c_stream_frames_checked_as_they_arrive(oracle, mode):
     s, dcs = _mixed(oracle)
     c = R.as_send_c(oracle, s)
-    a, sa, ba = _run(oracle, mode, c, lzjb=False)
-    b, sb, bb = _run(oracle, mode, c)
+    a, sa, ba = B._run(oracle, mode, c)
+    b, sb, bb = B._run(oracle, mode, c, lzjb=True)
     assert np.array_equal(a, b)
-    for k in B.TIMING:
-        sa.pop(k); sb.pop(k)
     assert sa == sb
     ncomp = _count(dcs, R.DC_LZJB) + _count(dcs, R.DC_ZLE)
     assert bb["lzjb_encoded"] == bb["zle_encoded"] == 0
     assert bb["frame_ok"] == ba["frame_ok"] + ncomp and bb["skipped"] == ba["skipped"] - ncomp
-    _, want = R.block_check_lzjb(oracle, c, mode=R.VERIFY if mode == "verify" else R.RECOMPRESS,
-                                 out=None if mode == "verify" else b)
-    _same(bb, want, B.COUNTERS)
+    B._same(bb, B._want(oracle, mode, c, b, lzjb=True)[1])
 
 
 def test_compress_and_decompress_are_unchanged(oracle):
     s, _ = _mixed(oracle)
-    c, _, _ = _run(oracle, "compress", s, lzjb=False)
+    c, _, _ = B._run(oracle, "compress", s)
     for mode, src in (("compress", s), ("decompress", c), ("recompress", s)):
-        a, sa, ba = _run(oracle, mode, src, lzjb=False, batch_bytes=1 << 18)
-        b, sb, bb = _run(oracle, mode, src, batch_bytes=1 << 18)
+        a, sa, ba = B._run(oracle, mode, src, batch_bytes=1 << 18)
+        b, sb, bb = B._run(oracle, mode, src, batch_bytes=1 << 18, lzjb=True)
         assert np.array_equal(a, b), mode
-        for k in B.TIMING:
-            sa.pop(k); sb.pop(k)
         assert sa == sb and ba == bb and bb["lzjb_encoded"] == bb["zle_encoded"] == 0, mode
 
 
 @pytest.mark.parametrize("chunk", [4093, 1 << 20])
 def test_ring_api(oracle, chunk):
     s, dcs = _mixed(oracle)
-    _, want = R.block_check_lzjb(oracle, s)
+    _, want = R.block_check(oracle, s, R.VERIFY, lzjb=True)
     for kw in (dict(batch_bytes=1 << 18), {}):
-        with _stage("verify", **kw) as g:
+        with B._stage("verify", lzjb=True, **kw) as g:
             out, err = B._pump(g, s.tobytes(), chunk)
             assert not err, err
             assert out == s.tobytes()
-            _same(g.block_stats(), want)
+            B._same(g.block_stats(), want)
             assert want["lzjb_encoded"] == _count(dcs, R.DC_LZJB) > 0
 
 
@@ -206,7 +179,7 @@ def device_api_subbatched(oracle, mem, nrec):
         recs, _ = index_host(src)
         d_in, p_in = mem.put(src)
         d_recs, p_recs = mem.put(recs.view(np.uint8))
-        with _stage("verify") as g:
+        with B._stage("verify", lzjb=True) as g:
             g.dev_submit(p_in, src.size, p_recs, len(recs))
             if fails:
                 with pytest.raises(MtzError) as ei:
@@ -214,9 +187,9 @@ def device_api_subbatched(oracle, mem, nrec):
                 assert ei.value.code == ECKSUM and g.stats()["bad_record"] == raw[-2]
             else:
                 g.dev_finish()
-                _, want = R.block_check_lzjb(oracle, src)
+                _, want = R.block_check(oracle, src, R.VERIFY, lzjb=True)
                 assert want["lzjb_encoded"] + want["zle_encoded"] == len(comp)
-                _same(g.block_stats(), want)
+                B._same(g.block_stats(), want)
 
 
 def test_device_api_across_the_subbatch_edge(oracle):
@@ -233,8 +206,8 @@ def test_deferred_shards(oracle):
     late = [i for i in comp if i > 31][0]
     for miss in (None, late):
         src = s if miss is None else B._corrupt_restamped(oracle, s, miss, byte=100)
-        _, want = R.block_check_lzjb(oracle, src)
-        gs = [_stage("verify", batch_bytes=1 << 18, flags=FLAG_DEFER_VERIFY) for _ in range(2)]
+        _, want = R.block_check(oracle, src, R.VERIFY, lzjb=True)
+        gs = [B._stage("verify", batch_bytes=1 << 18, flags=FLAG_DEFER_VERIFY, lzjb=True) for _ in range(2)]
         try:
             gs[0].process_host(src[:cut]); gs[1].process_host(src[cut:])
             a0 = gs[0].dev_aggregate()
@@ -256,9 +229,9 @@ def test_device_group(oracle):
     if torch.cuda.device_count() < 2:
         pytest.skip("needs two GPUs")
     s, _ = _mixed(oracle)
-    _, want = R.block_check_lzjb(oracle, s)
-    _, _, bs = _run(oracle, "verify", s, devices=[0, 1], batch_bytes=1 << 18)
-    _same(bs, want)
+    _, want = R.block_check(oracle, s, R.VERIFY, lzjb=True)
+    _, _, bs = B._run(oracle, "verify", s, devices=[0, 1], batch_bytes=1 << 18, lzjb=True)
+    B._same(bs, want)
 
 
 def test_real_streams_with_lzjb_or_zle_keys(oracle):
@@ -272,7 +245,7 @@ def test_real_streams_with_lzjb_or_zle_keys(oracle):
         if not keyed:
             continue
         found = True
-        _, st, bs = _run(oracle, "verify", s, block_sha256=True, block_sha512=True)
+        _, st, bs = B._run(oracle, "verify", s, sha256=True, sha512=True, lzjb=True)
         assert bs["frame_miss"] == 0, (p, bs)
     if not found:
         pytest.skip("no real stream with lzjb or zle keys under tests/golden/real")

@@ -9,14 +9,14 @@ import hashlib
 
 import pytest
 
-import block_frames_ref as R
+import block_ref as R
 from test_host_pipeline import _run_restore, fakezfs  # noqa: F401  (fixture)
 
 pytestmark = pytest.mark.gpu
 
 
 def test_lz4_on_disk_keys_in_verify_on_both_sides(fakezfs, tmp_path, oracle):  # noqa: F811
-    s, dcs = R.as_lz4_on_disk(oracle, fakezfs["stream"])
+    s, dcs = R.as_on_disk(oracle, fakezfs["stream"])
     nlz4 = sum(1 for v in dcs.values() if v == R.DC_LZ4)
     assert 0 < nlz4 <= len(dcs)
     p = tmp_path / "lz4.bin"

@@ -8,7 +8,7 @@ import hashlib
 
 import pytest
 
-import block_logical_ref as R
+import block_ref as R
 from test_host_pipeline import _run_restore, fakezfs  # noqa: F401  (fixture)
 
 pytestmark = pytest.mark.gpu

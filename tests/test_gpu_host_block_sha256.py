@@ -6,14 +6,14 @@ import hashlib
 
 import pytest
 
-import block_sha256_ref as R
+import block_ref as R
 from test_host_pipeline import _run_restore, fakezfs  # noqa: F401  (fixture)
 
 pytestmark = pytest.mark.gpu
 
 
 def test_sha256_keys_on_the_compressed_wire(fakezfs, tmp_path, oracle):  # noqa: F811
-    s = R.as_sha256(oracle, fakezfs["stream"])
+    s = R.as_sha(oracle, fakezfs["stream"], "sha256")
     p = tmp_path / "sha256.bin"
     s.tofile(str(p))
     env = {"FAKE_ZFS_STREAM": str(p)}

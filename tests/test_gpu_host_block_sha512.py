@@ -6,14 +6,14 @@ import hashlib
 
 import pytest
 
-import block_sha512_ref as R
+import block_ref as R
 from test_host_pipeline import _run_restore, fakezfs  # noqa: F401  (fixture)
 
 pytestmark = pytest.mark.gpu
 
 
 def test_sha512_keys_on_the_compressed_wire(fakezfs, tmp_path, oracle):  # noqa: F811
-    s = R.as_sha512(oracle, fakezfs["stream"])
+    s = R.as_sha(oracle, fakezfs["stream"], "sha512")
     p = tmp_path / "sha512.bin"
     s.tofile(str(p))
     env = {"FAKE_ZFS_STREAM": str(p)}

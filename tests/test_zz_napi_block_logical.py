@@ -12,7 +12,7 @@ import subprocess
 import numpy as np
 import pytest
 
-import block_logical_ref as R
+import block_ref as R
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 STUBS = os.path.join(ROOT, "tests", "stubs")

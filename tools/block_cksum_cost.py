@@ -5,7 +5,7 @@ flag off and on, the two handles alternating step by step so that both see the s
   verify      a 16 GiB uncompressed stream (128 KiB records): every block is checked logically
               against its key on the input's K1 sums
   recompress  the `zfs send -c` form of a 1 GiB stream whose keys say "written with
-              compression=lz4" (tests/block_cksum_ref.py): frames checked on the input
+              compression=lz4" (tests/block_ref.py): frames checked on the input
 
 Prints one JSON line (and writes it to --out): per workload the mean step time of each leg, the
 difference, the block counters, and the GPU name and power limit the numbers were taken on.
@@ -97,7 +97,7 @@ def main():
     if not torch.cuda.is_available():
         sys.exit("block_cksum_cost.py measures device time: it needs a GPU")
     import oracle as O
-    import block_cksum_ref as R
+    import block_ref as R
     O.build()
     nth = os.cpu_count() or 1
     result = {"tool": "block_cksum_cost", **gpu_info(), "steps": args.steps, "warmup": args.warmup}
@@ -107,7 +107,7 @@ def main():
     del s
     n = max(1, int(args.recompress_gib * (1 << 30)) // (RECSIZE + 312))
     raw = O.synth_stream(n, RECSIZE, O.PAYLOAD_PGPAGE, nthreads=nth)
-    disk, _ = R.as_lz4_on_disk(O, raw)
+    disk, _ = R.as_on_disk(O, raw)
     c = R.as_send_c(O, disk)
     result["recompress"] = time_legs("recompress", c, args.steps, args.warmup, raw.size + (1 << 20))
     line = json.dumps(result)

@@ -2,7 +2,7 @@
 """Cost of MTZ_FLAG_BLOCK_FRAMES (VERIFY encodes a frame for every raw block whose key covers an LZ4
 frame on disk: k_frame_plan, K3, k_frame_sums, kernels_frames.cuh), each leg against
 MTZ_FLAG_BLOCK_CKSUM alone on the same stream, the two handles alternating step by step so that both
-see the same machine.  Every stream is the generator's pg-page records re-keyed by as_lz4_on_disk()
+see the same machine.  Every stream is the generator's pg-page records re-keyed by as_on_disk()
 (ashift 9): what `zfs send` without -c carries for a dataset with compression=lz4.
 
   verify  a resident 16 GiB stream of 128 KiB records (device API, CUDA events): step time, and the
@@ -41,9 +41,9 @@ def _stage(mode, leg, **kw):
 
 
 def lz4_keyed(O, s, threads):
-    """as_lz4_on_disk(O, s) with the frames and their Fletcher-4 taken on `threads` threads"""
+    """as_on_disk(O, s) with the frames and their Fletcher-4 taken on `threads` threads"""
     import numpy as np
-    import block_frames_ref as R
+    import block_ref as R
     s = np.array(s, dtype=np.uint8, copy=True)
     todo = [(off, po, pl) for off, po, pl, t in R.records(s) if t == 3 and s[off + 50] == 0]
 

@@ -143,7 +143,7 @@ def main():
         sys.exit("block_logical_cost.py measures device time: it needs a GPU")
     import numpy as np
     import oracle as O
-    import block_logical_ref as R
+    import block_ref as R
     O.build()
     nth = os.cpu_count() or 1
     result = {"tool": "block_logical_cost", **gpu_info(), "steps": args.steps, "warmup": args.warmup}
@@ -164,7 +164,7 @@ def main():
     x = np.ascontiguousarray(raw(args.gib))
     result["recompress_raw_keys_fletcher4"] = resident_legs("recompress", R.send_c_form(O, x), args.steps,
                                                             args.warmup, args.profile_steps)
-    x = R.as_sha256(O, x, nth)
+    x = R.as_sha(O, x, "sha256", nth)
     result["recompress_raw_keys_sha256"] = resident_legs("recompress", R.send_c_form(O, x), args.steps, args.warmup,
                                                          args.profile_steps, block_sha256=True)
     del x

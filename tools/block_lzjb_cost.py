@@ -41,10 +41,10 @@ F._stage = _stage
 
 
 def keyed(O, s, threads, codec):
-    """block_lzjb_ref.as_on_disk(O, s, 9, codec) with the frames and their Fletcher-4 taken on `threads`
+    """block_ref.as_on_disk(O, s, 9, codec) with the frames and their Fletcher-4 taken on `threads`
     threads (the C restatement releases the GIL)"""
     import numpy as np
-    import block_lzjb_ref as R
+    import block_ref as R
     s = np.array(s, dtype=np.uint8, copy=True)
     todo = [(off, po, pl) for off, po, pl, t in R.records(s) if t == 3 and s[off + 50] == 0]
 
@@ -81,7 +81,7 @@ def main():
     if not torch.cuda.is_available():
         sys.exit("block_lzjb_cost.py measures device time: it needs a GPU")
     import oracle as O
-    import block_lzjb_ref as R
+    import block_ref as R
     O.build()
     nth = os.cpu_count() or 1
     result = {"tool": "block_lzjb_cost", **gpu_info(), "steps": args.steps, "warmup": args.warmup}

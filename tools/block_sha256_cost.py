@@ -165,15 +165,14 @@ def main(hash_name="sha256"):
     if not torch.cuda.is_available():
         sys.exit("block_%s_cost.py measures device time: it needs a GPU" % hash_name)
     import oracle as O
-    import block_sha512_ref as R
+    import block_ref as R
     O.build()
     nth = os.cpu_count() or 1
-    rekey = R.as_sha256 if hash_name == "sha256" else R.as_sha512
     result = {"tool": "block_%s_cost" % hash_name, **gpu_info(), "steps": args.steps, "warmup": args.warmup}
 
     rs = 131072
     n = max(1, int(args.verify_gib * (1 << 30)) // (rs + 312))
-    s = rekey(O, O.synth_stream(n, rs, O.PAYLOAD_PCG, nthreads=nth), threads=nth)
+    s = R.as_sha(O, O.synth_stream(n, rs, O.PAYLOAD_PCG, nthreads=nth), hash_name, threads=nth)
     v = resident_legs("verify", s, args.steps, args.warmup, 0, args.profile_steps)
     hashed = v["block_stats"][hash_name] // (args.steps + args.warmup) * (rs + blk)
     v["hashed_bytes_per_step"] = hashed
@@ -185,15 +184,15 @@ def main(hash_name="sha256"):
     result["host"] = {}
     for rs in (131072, 1 << 20):
         n = max(1, int(args.host_gib * (1 << 30)) // (rs + 312))
-        s = rekey(O, O.synth_stream(n, rs, O.PAYLOAD_PCG, nthreads=nth), threads=nth)
+        s = R.as_sha(O, O.synth_stream(n, rs, O.PAYLOAD_PCG, nthreads=nth), hash_name, threads=nth)
         result["host"]["recsize_%d" % rs] = host_legs(s, args.host_steps, 1)
         del s
 
     rs = 131072
     n = max(1, int(args.recompress_gib * (1 << 30)) // (rs + 312))
     raw = O.synth_stream(n, rs, O.PAYLOAD_PGPAGE, nthreads=nth)
-    disk, _ = R.as_lz4_on_disk(O, raw)
-    c = R.as_send_c(O, rekey(O, disk, threads=nth))
+    disk, _ = R.as_on_disk(O, raw)
+    c = R.as_send_c(O, R.as_sha(O, disk, hash_name, threads=nth))
     result["recompress"] = resident_legs("recompress", c, args.steps, args.warmup, raw.size + (1 << 20),
                                          args.profile_steps)
     line = json.dumps(result)
