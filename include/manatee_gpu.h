@@ -117,6 +117,19 @@ extern "C" {
                                   * change; mtz_block_stats.logical_checked counts these records.  VERIFY
                                   * accepts the flag and does not change */
 
+#define MTZ_FLAG_LZ4_HC 256u     /* COMPRESS: encode the DRR_WRITE payloads with the stage's high-ratio LZ4
+                                  * encoder (a 16-way hash chain, DESIGN.md section 1) instead of ZFS's
+                                  * fast one; about 10 % fewer payload bytes on the wire for pg-like pages.
+                                  * Every frame is a valid ZFS-LZ4 frame that any DECOMPRESS stage (and
+                                  * LZ4_decompress_safe) decodes; the wire format does not change.  The
+                                  * block check compares LZ4-keyed records with these frames, so they
+                                  * nearly always count as frame_miss (never an error).  Device scratch
+                                  * for the hash tables: 256 KiB x 4 x SM count (132 MiB on a 132-SM
+                                  * H100) per batch in flight, i.e. n_slots x devices of them for the
+                                  * ring API and mtz_process_host, two for the device API.  VERIFY,
+                                  * DECOMPRESS, RECOMPRESS and PASSTHROUGH accept the flag and do not
+                                  * change */
+
 typedef struct mtz_handle mtz_handle;
 
 #define MTZ_MAX_DEVICES 16
@@ -350,6 +363,10 @@ int32_t mtz_set_carry(mtz_handle *h, const uint64_t carry_in[4],
 int32_t mtz_k_lz4_decode(mtz_handle *h, const void *d_src, void *d_dst,
     mtz_job *d_jobs, uint32_t njobs, void *cuda_stream);
 int32_t mtz_k_lz4_encode(mtz_handle *h, const void *d_src, void *d_dst,
+    mtz_job *d_jobs, uint32_t njobs, void *cuda_stream);
+/* the MTZ_FLAG_LZ4_HC encoder (K3h) on any handle, same contract as mtz_k_lz4_encode; its hash
+ * tables (132 MiB on a 132-SM H100) are allocated on the first call and freed by mtz_close */
+int32_t mtz_k_lz4hc_encode(mtz_handle *h, const void *d_src, void *d_dst,
     mtz_job *d_jobs, uint32_t njobs, void *cuda_stream);
 
 #ifdef __cplusplus

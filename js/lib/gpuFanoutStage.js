@@ -58,7 +58,8 @@ function GpuFanoutStage(options) {
             (options.blockSha512 ? 16 : 0) |       // gpu.blockSha512: MTZ_FLAG_BLOCK_SHA512
             (options.blockFrames ? 32 : 0) |       // gpu.blockFrames: MTZ_FLAG_BLOCK_FRAMES
             (options.blockLzjb ? 64 : 0) |         // gpu.blockLzjb: MTZ_FLAG_BLOCK_LZJB
-            (options.blockLogical ? 128 : 0)       // gpu.blockLogical: MTZ_FLAG_BLOCK_LOGICAL
+            (options.blockLogical ? 128 : 0) |     // gpu.blockLogical: MTZ_FLAG_BLOCK_LOGICAL
+            (options.lz4Hc ? 256 : 0)              // gpu.lz4Hc: MTZ_FLAG_LZ4_HC
     });
     this._blockChecksums = !!options.blockChecksums;
     this._peers = [];

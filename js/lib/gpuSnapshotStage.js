@@ -25,6 +25,7 @@ var BLOCK_SHA512 = 16;      // MTZ_FLAG_BLOCK_SHA512 (with BLOCK_CKSUM only)
 var BLOCK_FRAMES = 32;      // MTZ_FLAG_BLOCK_FRAMES (with BLOCK_CKSUM only)
 var BLOCK_LZJB = 64;        // MTZ_FLAG_BLOCK_LZJB (with BLOCK_CKSUM only)
 var BLOCK_LOGICAL = 128;    // MTZ_FLAG_BLOCK_LOGICAL (with BLOCK_CKSUM only)
+var LZ4_HC = 256;           // MTZ_FLAG_LZ4_HC (COMPRESS; the other modes accept it)
 
 function GpuSnapshotStage(options) {
     if (!(this instanceof GpuSnapshotStage)) {
@@ -46,7 +47,8 @@ function GpuSnapshotStage(options) {
             (options.blockSha512 ? BLOCK_SHA512 : 0) |       // gpu.blockSha512
             (options.blockFrames ? BLOCK_FRAMES : 0) |       // gpu.blockFrames
             (options.blockLzjb ? BLOCK_LZJB : 0) |           // gpu.blockLzjb
-            (options.blockLogical ? BLOCK_LOGICAL : 0)       // gpu.blockLogical
+            (options.blockLogical ? BLOCK_LOGICAL : 0) |     // gpu.blockLogical
+            (options.lz4Hc ? LZ4_HC : 0)                     // gpu.lz4Hc
     });
     this._blockChecksums = !!options.blockChecksums;
     this._pending = null;      // {chunk, off, cb} waiting for ring space

@@ -23,6 +23,7 @@ FLAG_BLOCK_SHA512 = 16
 FLAG_BLOCK_FRAMES = 32
 FLAG_BLOCK_LZJB = 64
 FLAG_BLOCK_LOGICAL = 128
+FLAG_LZ4_HC = 256
 XCHG_FIRST, XCHG_LAST = 1, 2
 MODE_NAMES = {"verify": 0, "compress": 1, "decompress": 2, "recompress": 3, "passthrough": 4}
 
@@ -78,7 +79,7 @@ SYMBOLS = [
     "mtz_get_block_stats", "mtz_end_checksum", "mtz_host_alloc", "mtz_host_free", "mtz_process_host",
     "mtz_index_host", "mtz_dev_index", "mtz_dev_submit", "mtz_dev_aggregate",
     "mtz_dev_finish", "mtz_dev_reset", "mtz_dev_aggregate_async", "mtz_dev_finish_gathered", "mtz_set_carry",
-    "mtz_k_lz4_decode", "mtz_k_lz4_encode",
+    "mtz_k_lz4_decode", "mtz_k_lz4_encode", "mtz_k_lz4hc_encode",
     "mtz_fanout_attach", "mtz_out_peek_peer", "mtz_out_consume_peer", "mtz_read_peer", "mtz_cancel",
     "mtz_comm_unique_id", "mtz_comm_init", "mtz_comm_share", "mtz_dev_finish_exchange",
 ]
@@ -154,6 +155,7 @@ def lib():
                                           C.POINTER(u64 * 4), C.POINTER(u64 * 4)]
     L.mtz_k_lz4_decode.argtypes = [H, vp, vp, vp, C.c_uint32, vp]
     L.mtz_k_lz4_encode.argtypes = [H, vp, vp, vp, C.c_uint32, vp]
+    L.mtz_k_lz4hc_encode.argtypes = [H, vp, vp, vp, C.c_uint32, vp]
     for s in SYMBOLS:
         getattr(L, s).restype = getattr(L, s).restype if s in (
             "mtz_last_error", "mtz_strerror") else i32

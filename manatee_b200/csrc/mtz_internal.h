@@ -12,6 +12,7 @@
 #include "../../include/manatee_gpu.h"
 #include "kernels_fletcher.cuh"
 #include "kernels_lz4.cuh"
+#include "kernels_lz4hc.cuh"
 #include "kernels_codec.cuh"
 #include "kernels_index.cuh"
 #include "kernels_block.cuh"
@@ -58,6 +59,7 @@ struct CodecBufs {
 	uint8_t *d_logical = nullptr, *d_enc = nullptr;
 	uint32_t *seq_n = nullptr, *cert = nullptr;         // RECOMPRESS certificate: K2's parse sizes, K3c's verdicts
 	uint32_t *k3_skip = nullptr;                        // VERIFY with BLOCK_FRAMES and BLOCK_LZJB: K3 leaves these jobs
+	uint32_t *hc_tab = nullptr;                         // COMPRESS with MTZ_FLAG_LZ4_HC: K3h's hash tables (hc_tab_bytes)
 	mtz_job *chk = nullptr;                             // BLOCK_LOGICAL: k_logical_plan's jobs
 	RecSums *chk_sums = nullptr;                        // ... and the sums of their bytes
 	uint8_t *d_chk = nullptr;                           // ... with BLOCK_LZJB: the slots of the lzjb / zle frames
@@ -125,6 +127,7 @@ struct mtz_handle {
 	mtz_config cfg{};
 	int device = 0;
 	int sm_count = 0;
+	uint32_t *k_hc_tab = nullptr;      // mtz_k_lz4hc_encode's hash tables (allocated on first use)
 	std::string err;
 	std::mutex err_mu;
 	std::atomic<int32_t> failed{0};

@@ -414,6 +414,7 @@ int32_t mtz_close(mtz_handle *h)
 		codec_free(h->dv_cb2);
 	}
 	codec_free(h->dv_cb);
+	if (h->k_hc_tab) cudaFree(h->k_hc_tab);
 	if (h->st_post) cudaStreamDestroy(h->st_post);
 	if (h->st_dec) cudaStreamDestroy(h->st_dec);
 	for (int i = 0; i < 2; i++) {
@@ -630,6 +631,8 @@ static int32_t launch_block(mtz_handle *h, cudaStream_t st, const uint8_t *d_in,
 
 static int32_t launch_k3(mtz_handle *h, cudaStream_t st, const void *d_src, void *d_dst,
     mtz_job *d_jobs, uint32_t njobs, bool compact, const uint32_t *skip = nullptr, bool count = true);
+static int32_t launch_k3h(mtz_handle *h, cudaStream_t st, const void *d_src, void *d_dst,
+    mtz_job *d_jobs, uint32_t njobs, uint32_t *tabs);
 
 // The block check of a VERIFY (sub-)batch with MTZ_FLAG_BLOCK_FRAMES and/or MTZ_FLAG_BLOCK_LZJB: plan,
 // K3 (LZ4 jobs, with BLOCK_FRAMES), k_lzjb_encode and k_zle_encode (lzjb / zle jobs, with BLOCK_LZJB)
@@ -767,6 +770,19 @@ static bool certify_on(const mtz_handle *h)
 	return on && h->cfg.mode == MTZ_MODE_RECOMPRESS && !(h->cfg.flags & MTZ_FLAG_REENCODE_ALL);
 }
 
+// COMPRESS with MTZ_FLAG_LZ4_HC encodes with K3h (kernels_lz4hc.cuh) instead of K3; the other modes
+// accept the flag and do not change
+static bool lz4hc_on(const mtz_handle *h)
+{
+	return h->cfg.mode == MTZ_MODE_COMPRESS && (h->cfg.flags & MTZ_FLAG_LZ4_HC) != 0;
+}
+
+// K3h's hash tables: one per warp of its persistent grid (launch_k3h)
+static size_t hc_tab_bytes(const mtz_handle *h)
+{
+	return (size_t)h->sm_count * LZ4HC_CTAS_PER_SM * LZ4HC_WARPS * LZ4HC_TAB_BYTES;
+}
+
 static int32_t codec_alloc(mtz_handle *h, CodecBufs &cb, size_t rec_cap, size_t scratch_cap)
 {
 	cb.rec_cap = rec_cap; cb.scratch_cap = scratch_cap;
@@ -784,6 +800,7 @@ static int32_t codec_alloc(mtz_handle *h, CodecBufs &cb, size_t rec_cap, size_t 
 	if (h->cfg.mode != MTZ_MODE_DECOMPRESS) MTZ_CU(h, cudaMalloc(&cb.d_enc, scratch_cap + 512));
 	if (h->cfg.mode == MTZ_MODE_VERIFY && block_lzjb_on(h) && (h->cfg.flags & MTZ_FLAG_BLOCK_FRAMES))
 		MTZ_CU(h, cudaMalloc(&cb.k3_skip, rec_cap * sizeof(uint32_t)));
+	if (lz4hc_on(h)) MTZ_CU(h, cudaMalloc(&cb.hc_tab, hc_tab_bytes(h)));
 	if (block_logical_on(h)) {
 		MTZ_CU(h, cudaMalloc(&cb.chk, rec_cap * sizeof(mtz_job)));
 		MTZ_CU(h, cudaMalloc(&cb.chk_sums, rec_cap * sizeof(RecSums)));
@@ -810,7 +827,7 @@ static void codec_free(CodecBufs &cb)
 	cudaFree(cb.cr); cudaFree(cb.vals); cudaFree(cb.offs); cudaFree(cb.out_offs);
 	cudaFree(cb.dec); cudaFree(cb.enc); cudaFree(cb.out_recs); cudaFree(cb.osums); cudaFree(cb.steps);
 	cudaFree(cb.d_logical); cudaFree(cb.d_enc); cudaFree(cb.d_cres); cudaFree(cb.d_ores);
-	cudaFree(cb.d_outpos); cudaFree(cb.seq_n); cudaFree(cb.cert); cudaFree(cb.k3_skip);
+	cudaFree(cb.d_outpos); cudaFree(cb.seq_n); cudaFree(cb.cert); cudaFree(cb.k3_skip); cudaFree(cb.hc_tab);
 	cudaFree(cb.chk); cudaFree(cb.chk_sums); cudaFree(cb.d_chk); cudaFree(cb.chk_pos);
 	if (cb.h_cres) cudaFreeHost(cb.h_cres);
 	if (cb.h_ores) cudaFreeHost(cb.h_ores);
@@ -890,8 +907,12 @@ static int32_t codec_launch_enc(mtz_handle *h, cudaStream_t st, CodecBufs &cb, s
 	if (ka) MTZ_CU(h, cudaEventRecord(ka, st));
 	if (st_k3 != st) MTZ_CU(h, cudaStreamWaitEvent(st_k3, ka, 0));
 	int32_t rc = MTZ_OK;
-	if (cb.cert != nullptr) rc = launch_k3c(h, st_k3, cb, (uint32_t)nrec, compact);
-	if (rc == MTZ_OK) rc = launch_k3(h, st_k3, nullptr, nullptr, cb.enc, (uint32_t)nrec, compact, cb.cert);
+	if (cb.hc_tab != nullptr) {
+		rc = launch_k3h(h, st_k3, nullptr, nullptr, cb.enc, (uint32_t)nrec, cb.hc_tab);
+	} else {
+		if (cb.cert != nullptr) rc = launch_k3c(h, st_k3, cb, (uint32_t)nrec, compact);
+		if (rc == MTZ_OK) rc = launch_k3(h, st_k3, nullptr, nullptr, cb.enc, (uint32_t)nrec, compact, cb.cert);
+	}
 	if (rc == MTZ_OK && kb) MTZ_CU(h, cudaEventRecord(kb, st_k3));
 	if (rc == MTZ_OK && st_k3 != st) MTZ_CU(h, cudaStreamWaitEvent(st, kb, 0));
 	return rc;
@@ -1952,6 +1973,31 @@ int32_t mtz_k_lz4_encode(mtz_handle *h, const void *d_src, void *d_dst, mtz_job 
 	// MTZ_K3_FORCE_COMPACT: the caller vouches that every job is a 128 KiB-class block (experiments)
 	const char *e = getenv("MTZ_K3_FORCE_COMPACT");
 	return launch_k3(h, st, d_src, d_dst, d_jobs, njobs, e != nullptr && atoi(e) != 0);
+}
+
+// K3h over njobs jobs with `tabs` (hc_tab_bytes): the persistent grid has exactly the warps the
+// tables were sized for, at most
+static int32_t launch_k3h(mtz_handle *h, cudaStream_t st, const void *d_src, void *d_dst,
+    mtz_job *d_jobs, uint32_t njobs, uint32_t *tabs)
+{
+	if (njobs == 0) return MTZ_OK;
+	const uint32_t need = (njobs + LZ4HC_WARPS - 1) / LZ4HC_WARPS;
+	const int grid = (int)std::min(need, (uint32_t)h->sm_count * (uint32_t)LZ4HC_CTAS_PER_SM);
+	k3h_lz4hc_encode<<<grid, LZ4HC_THREADS, 0, st>>>((const uint8_t *)d_src, (uint8_t *)d_dst, d_jobs, njobs, tabs);
+	MTZ_CU(h, cudaGetLastError());
+	count_launch(h, 1);
+	return MTZ_OK;
+}
+
+int32_t mtz_k_lz4hc_encode(mtz_handle *h, const void *d_src, void *d_dst, mtz_job *d_jobs,
+    uint32_t njobs, void *cuda_stream)
+{
+	CHECK_H(h);
+	if (njobs == 0) return MTZ_OK;
+	MTZ_CU(h, cudaSetDevice(h->device));
+	cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : h->st;
+	if (h->k_hc_tab == nullptr) MTZ_CU(h, cudaMalloc(&h->k_hc_tab, hc_tab_bytes(h)));
+	return launch_k3h(h, st, d_src, d_dst, d_jobs, njobs, h->k_hc_tab);
 }
 
 // ------------------------------------------------------- GPU-side parse ---

@@ -136,7 +136,8 @@ class BackupSender(object):
                                 block_sha512=bool(g.get("blockSha512")),
                                 block_frames=bool(g.get("blockFrames")),
                                 block_lzjb=bool(g.get("blockLzjb")),
-                                block_logical=bool(g.get("blockLogical")))
+                                block_logical=bool(g.get("blockLogical")),
+                                lz4_hc=bool(g.get("lz4Hc")))
 
     def _stage_stats(self, stage):
         """job.gpu: the stage counters, plus `blocks` (block-checksum counters) with

@@ -21,7 +21,8 @@ class GpuSnapshotStage(object):
 
     def __init__(self, mode="verify", device=0, ring_bytes=0, batch_bytes=0, n_slots=0,
                  out_ring_bytes=0, flags=0, devices=None, block_checksums=False, block_sha256=False,
-                 block_sha512=False, block_frames=False, block_lzjb=False, block_logical=False):
+                 block_sha512=False, block_frames=False, block_lzjb=False, block_logical=False,
+                 lz4_hc=False):
         """``devices`` = CUDA ordinals of a device group: the GPUs of one box run as ONE stage,
         batch b of the stream on ``devices[b % len(devices)]`` (mtz_config.devices[]).
         ``block_checksums`` = MTZ_FLAG_BLOCK_CKSUM: every DRR_WRITE is also checked against the
@@ -44,7 +45,10 @@ class GpuSnapshotStage(object):
         the decoded bytes (ECKSUM on a mismatch), with ``block_lzjb`` the three modes encode lzjb / zle
         frames of raw and LZ4 records as VERIFY does, and DECOMPRESS counts a raw record with an LZ4
         key as the frame miss the sender counted (``block_stats()["logical_checked"]``).  VERIFY
-        accepts it and does not change.  Only valid with ``block_checksums``."""
+        accepts it and does not change.  Only valid with ``block_checksums``.
+        ``lz4_hc`` = MTZ_FLAG_LZ4_HC: COMPRESS encodes with the stage's high-ratio LZ4 encoder (about
+        10 % fewer payload bytes on the wire for pg-like pages, frames any DECOMPRESS stage decodes);
+        the other modes accept it and do not change."""
         if block_checksums:
             flags |= N.FLAG_BLOCK_CKSUM
         if block_sha256:
@@ -57,6 +61,8 @@ class GpuSnapshotStage(object):
             flags |= N.FLAG_BLOCK_LZJB
         if block_logical:
             flags |= N.FLAG_BLOCK_LOGICAL
+        if lz4_hc:
+            flags |= N.FLAG_LZ4_HC
         self._L = N.lib()
         self._h = C.c_void_p()
         cfg = N.Config()

@@ -46,6 +46,7 @@ PARAMS = {
     "test_the_compressed_wire_counts_what_verify_counts": [(dict(sha256=False, sha512=False, lzjb=False),),
                                                            (dict(sha256=True, sha512=True, lzjb=True),)],
     "test_a_corrupted_raw_keyed_lz4_record_fails_the_recompress_relay": [("fletcher4",), ("sha256",), ("sha512",)],
+    "test_block_check_counts_the_hc_frames": [(False,), (True,)],
 }
 SKIP = {"test_sixteen_mib_record": "16 MiB blocks take minutes per encode on the emulator",
         "test_size_independent_properties_at_2gib": "2 GiB of LZ4 work is out of reach for the emulator",
@@ -54,6 +55,10 @@ SKIP = {"test_sixteen_mib_record": "16 MiB blocks take minutes per encode on the
         "test_deferred_codec_shards": "its device buffers are torch tensors; tests/test_emul_block_logical.py runs it "
                                       "on host memory",
         "test_device_group": "needs two GPUs",
+        "test_fanout_of_two_peers": "needs two GPUs",
+        "test_kernel_equals_the_oracle_on_thousands_of_jobs": "3000 jobs and a 16 MiB block take hours on the emulator; "
+                                                              "tests/test_emul_lz4hc.py runs K3h inside guard pages",
+        "test_host_pipeline_compress_hc_to_a_plain_decompress": "needs the fake-zfs fixture (pytest)",
         "test_real_streams_with_lzjb_or_zle_keys": "tests/golden/real holds no stream with lzjb or zle keys"}
 
 
@@ -75,10 +80,11 @@ def main():
     import test_gpu_block_logical as L
     import test_gpu_codec as K
     import test_gpu_lz4 as Z
+    import test_gpu_lz4hc as HC
     import test_gpu_stream as S
     import test_gpu_verify as V
     tot = fail = 0
-    for mod in (V, S, Z, K, B, H, W, F, J, L):
+    for mod in (V, S, Z, K, B, H, W, F, J, L, HC):
         for name, fn in inspect.getmembers(mod, inspect.isfunction):
             if not name.startswith("test_") or filt not in name:
                 continue
