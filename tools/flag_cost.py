@@ -1,0 +1,417 @@
+#!/usr/bin/env python
+"""What a flag of GpuSnapshotStage costs on the GPU, one subcommand per workload.  Every measurement
+runs the same stream through two handles, the baseline leg and the flag leg, alternating step by step so
+that both see the same machine, and prints one JSON line (and writes it to --out) with the GPU name,
+power limit and max SM clock the numbers were taken on.
+
+  block_cksum    MTZ_FLAG_BLOCK_CKSUM off / on: resident VERIFY of 16 GiB of uncompressed 128 KiB
+                 records, resident RECOMPRESS of the `zfs send -c` form of 1 GiB with "LZ4 on disk" keys
+  block_sha256   MTZ_FLAG_BLOCK_SHA256 against MTZ_FLAG_BLOCK_CKSUM alone on streams with SHA-256 keys:
+                 resident VERIFY (with k_block_sha256's device time and the bytes it hashes per second),
+                 mtz_process_host VERIFY with 128 KiB and 1 MiB records (SHA-256 is serial per record, so
+                 1 MiB records give the kernel few threads and show the latency of one hash), resident
+                 RECOMPRESS of the `send -c` form
+  block_sha512   the same for MTZ_FLAG_BLOCK_SHA512 on streams with SHA-512 keys
+  block_frames   MTZ_FLAG_BLOCK_FRAMES against MTZ_FLAG_BLOCK_CKSUM alone on pg-page records keyed as ZFS
+                 with compression=lz4 at ashift 9 writes them, sent without -c: resident VERIFY, host
+                 VERIFY with 128 KiB and 1 MiB records at 32 MiB and 256 MiB batches, and the ring API
+                 (acquire + commit, bench.py's ring_run) at each leg's default batch size
+  block_lzjb     the same for MTZ_FLAG_BLOCK_LZJB on lzjb-keyed records, plus resident VERIFY of
+                 zle-keyed ones
+  block_logical  MTZ_FLAG_BLOCK_LOGICAL against the same flags without it: resident COMPRESS and
+                 DECOMPRESS of lzjb-keyed records (at --gib and at --large-gib), resident RECOMPRESS of
+                 the compressed form of raw-keyed records (fletcher4 and sha256 keys), host COMPRESS
+  lz4hc          MTZ_FLAG_LZ4_HC against COMPRESS without it: wire bytes, ratio and time, resident and host
+
+A resident step is timed with CUDA events around dev_submit + dev_finish on a side stream, a host pass
+with the host clock around mtz_process_host; kernel device times come from torch.profiler in a pass of
+their own.  Every counter is one pass's: resident legs dev_reset before every step (outside the timed
+window), host legs divide by the passes the handle ran; the first_* indices are reported as read.
+usage: tools/flag_cost.py WORKLOAD [options] [--out F]    (tools/flag_cost.py WORKLOAD -h lists them)"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+from concurrent.futures import ThreadPoolExecutor
+from contextlib import ExitStack, contextmanager
+from functools import partial
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+
+import block_ref as R  # noqa: E402
+import oracle as O  # noqa: E402
+
+RECSIZE = 131072
+NTH = os.cpu_count() or 1
+# the hash kernel of each SHA flag and its compression block: a 128 KiB record hashes 128 KiB + one
+# padding block
+HASHES = {"sha256": ("k_block_sha256", 64), "sha512": ("k_block_sha512", 128)}
+
+
+def gpu_info():
+    import torch
+    info = {"gpu": torch.cuda.get_device_name(0)}
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, timeout=30)
+        info["power_limit_and_max_sm_clock"] = q.stdout.strip().splitlines()[0] if q.stdout.strip() else None
+    except (OSError, subprocess.SubprocessError):
+        info["power_limit_and_max_sm_clock"] = None
+    return info
+
+
+def pair(base, flag, **shared):
+    """a leg pair: the baseline leg and the flag leg, each (name, GpuSnapshotStage keyword arguments),
+    and the keyword arguments both legs share -> {name: keyword arguments}, the baseline first"""
+    return {name: {**shared, **kw} for name, kw in (base, flag)}
+
+
+@contextmanager
+def stages(mode, legs):
+    from manatee_b200 import GpuSnapshotStage
+    with ExitStack() as es:
+        yield {name: es.enter_context(GpuSnapshotStage(mode, **kw)) for name, kw in legs.items()}
+
+
+def alternate(legs, passes):
+    """(pass, leg name) for `passes` passes of every leg, the order swapped every pass"""
+    names = list(legs)
+    for i in range(passes):
+        for name in (names if i % 2 == 0 else names[::-1]):
+            yield i, name
+
+
+def summary(legs, ms, nbytes=0, rate="gbps"):
+    """the step times of a leg pair; with `nbytes` also each leg's <leg>_<rate> in GB/s"""
+    base, flag = legs
+    res = {}
+    for name in legs:
+        v = sorted(ms[name])
+        res.update({name + "_ms_mean": sum(v) / len(v), name + "_ms_median": v[len(v) // 2],
+                    name + "_ms_min": v[0], name + "_ms_max": v[-1]})
+        if nbytes:
+            res[name + "_" + rate] = nbytes / (res[name + "_ms_mean"] * 1e6)
+    res["diff_ms_mean"] = res[flag + "_ms_mean"] - res[base + "_ms_mean"]
+    res["diff_pct_mean"] = 100.0 * res["diff_ms_mean"] / res[base + "_ms_mean"]
+    return res
+
+
+def leg_fields(gs, counters, passes, fields, out_bytes):
+    """the block counters of the legs named in `counters` (None: the flag leg) per pass, the flag leg's
+    as block_stats and a baseline's as <leg>_block_stats, and fields(name, stage, output bytes) of
+    every leg"""
+    flag = list(gs)[1]
+    res = {}
+    for name in ((flag,) if counters is None else counters):
+        st = gs[name].block_stats()
+        res["block_stats" if name == flag else name + "_block_stats"] = {
+            k: v if k.startswith("first_") else v // passes for k, v in st.items()}
+    for name, g in gs.items():
+        res.update(fields(name, g, out_bytes[name]) if fields else {})
+    return res
+
+
+def kernel_times(fn, n, kernels):
+    """device ms and launches per step of each of `kernels` over n calls of fn (torch.profiler, CUDA
+    activities)"""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(n):
+            fn()
+        torch.cuda.synchronize()
+    res = {}
+    for kern in kernels:
+        us, calls = 0.0, 0
+        for e in prof.key_averages():
+            if kern in e.key:
+                us += getattr(e, "device_time_total", None) or getattr(e, "cuda_time_total", 0.0)
+                calls += e.count
+        res[kern + "_ms_per_step"] = us / 1000.0 / n
+        res[kern + "_launches_per_step"] = calls / n
+    return res
+
+
+def resident(a, mode, s, legs, kernels=(), counters=None, fields=None, rate=None, same_output=True):
+    """ms per resident step of `mode` over the plain stream `s` held in HBM, on both legs of `legs`;
+    then the device time of `kernels` on the flag leg over --profile-steps steps.  When the mode writes
+    an output and both legs must write the same bytes, outputs_equal compares their last steps'."""
+    import numpy as np
+    import torch
+    from manatee_b200 import index_host
+    recs, used = index_host(s)
+    assert used == s.size
+    d_in = torch.empty(s.size + 512, dtype=torch.uint8, device="cuda")
+    d_in[:s.size].copy_(torch.from_numpy(s))
+    d_recs = torch.from_numpy(recs.view(np.uint8).copy()).cuda()
+    # the re-encoding modes' worst case (mtz_dev_submit's check) and a margin
+    cap = 0 if mode == "verify" else int(np.maximum(recs["lsize"], recs["payload"]).sum()) + 312 * len(recs) + (1 << 20)
+    d_out = torch.empty(cap, dtype=torch.uint8, device="cuda") if cap else None
+    st = torch.cuda.Stream()
+    ms, outs = {name: [] for name in legs}, {}
+    with stages(mode, legs) as gs:
+        def step(g):
+            g.dev_reset()
+            torch.cuda.synchronize()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(st)
+            g.dev_submit(d_in.data_ptr(), s.size, d_recs.data_ptr(), len(recs),
+                         d_out.data_ptr() if cap else 0, cap, cuda_stream=st.cuda_stream)
+            ob = g.dev_finish()[0]
+            e1.record(st)
+            torch.cuda.synchronize()
+            return e0.elapsed_time(e1), ob
+
+        for i, name in alternate(legs, a.warmup + a.steps):
+            t, ob = step(gs[name])
+            if i >= a.warmup:
+                ms[name].append(t)
+            if i == a.warmup + a.steps - 1:
+                # records are 8-byte aligned
+                outs[name] = (ob, d_out[:ob].view(torch.int64).sum().item() if cap else 0)
+        res = summary(legs, ms, s.size if rate else 0, rate)
+        res.update(leg_fields(gs, counters, 1, fields, {name: o[0] for name, o in outs.items()}))
+        res["records"] = int(len(recs))
+        res["stream_bytes"] = int(s.size)
+        base, flag = legs
+        if cap and same_output:
+            res["outputs_equal"] = outs[base] == outs[flag]
+        if kernels and a.profile_steps:
+            res.update(kernel_times(partial(step, gs[flag]), a.profile_steps, kernels))
+            res["profile_steps"] = a.profile_steps
+        return res
+
+
+def host(a, mode, s, legs, counters=None, fields=None, rate="gbps"):
+    """wall ms per mtz_process_host pass of the whole stream `s`, 1 warm-up and --host-steps timed
+    passes of both legs"""
+    import numpy as np
+    out = None if mode == "verify" else np.zeros(s.size + (64 << 20), dtype=np.uint8)
+    ms, obs = {name: [] for name in legs}, {}
+    with stages(mode, legs) as gs:
+        for i, name in alternate(legs, 1 + a.host_steps):
+            t0 = time.perf_counter()
+            obs[name] = gs[name].process_host(s, out)
+            dt = (time.perf_counter() - t0) * 1e3
+            assert out is not None or obs[name] == s.size
+            if i >= 1:
+                ms[name].append(dt)
+        res = summary(legs, ms, s.size, rate)
+        res.update(leg_fields(gs, counters, 1 + a.host_steps, fields, obs))
+        res["stream_bytes"] = int(s.size)
+        return res
+
+
+def ring(a, s, legs):
+    """GB/s of VERIFY through the ring API, acquire + commit (bench.py's ring_run with its native
+    producer), each pass of each leg on a fresh handle at its default batch size"""
+    import bench
+    from manatee_b200 import GpuSnapshotStage
+    base, flag = legs
+    secs, stats = {name: [] for name in legs}, {}
+    for _, name in alternate(legs, a.ring_steps):
+        with GpuSnapshotStage("verify", **legs[name]) as g:
+            dt, ok, detail = bench.ring_run(g, s, producer="acquire", nthreads=bench.pump_threads())
+            assert ok, detail
+            secs[name].append(dt)
+            stats[name] = g.block_stats()
+    res = {}
+    for name in legs:
+        v = sorted(secs[name])
+        res.update({name + "_gbps_mean": s.size / (sum(v) / len(v)) / 1e9, name + "_gbps_min": s.size / v[-1] / 1e9,
+                    name + "_gbps_max": s.size / v[0] / 1e9})
+    res["diff_pct_mean"] = 100.0 * (res[flag + "_gbps_mean"] / res[base + "_gbps_mean"] - 1.0)
+    res["block_stats"] = stats[flag]
+    res["stream_bytes"] = int(s.size)
+    res["steps"] = a.ring_steps
+    return res
+
+
+def synth(gib, kind, rs=RECSIZE):
+    """the generator's stream of about `gib` GiB of `rs`-byte records"""
+    return O.synth_stream(max(1, int(gib * (1 << 30)) // (rs + 312)), rs, kind, nthreads=NTH)
+
+
+def keyed(O, s, threads, codec):
+    """block_ref.as_on_disk(O, s, 9, codec)[0] for codec DC_LZ4, DC_LZJB or DC_ZLE, with the frames and
+    their Fletcher-4 taken on `threads` threads (the C encoders and checksum release the GIL)"""
+    import numpy as np
+    s = np.array(s, dtype=np.uint8, copy=True)
+    todo = [(off, po, pl) for off, po, pl, t in R.records(s) if t == 3 and s[off + 50] == 0]
+
+    def key(job):
+        _, po, pl = job
+        logical = s[po:po + pl]
+        fr = R.disk_frame(O, logical, 9, codec)
+        if fr is None:
+            return O.fletcher4(logical), R.prop(pl, pl, R.DC_OFF)
+        return O.fletcher4(np.ascontiguousarray(fr)), R.prop(pl, fr.size, codec)
+
+    with ThreadPoolExecutor(threads) as ex:
+        keys = list(ex.map(key, todo, chunksize=256))
+    for (off, _, _), (k, p) in zip(todo, keys):
+        R.set_key(s, off, R.FLETCHER4, k, p)
+    assert O.stream_restamp(s)[0] == 0
+    return s
+
+
+# ---- the workloads ------------------------------------------------------------------------------------
+
+def block_cksum(a):
+    legs = pair(("off", {}), ("on", {"block_checksums": True}))
+    c = R.as_send_c(O, keyed(O, synth(a.recompress_gib, O.PAYLOAD_PGPAGE), NTH, R.DC_LZ4))
+    return {"verify": resident(a, "verify", synth(a.verify_gib, O.PAYLOAD_PCG), legs),
+            "recompress": resident(a, "recompress", c, legs)}
+
+
+def block_sha(a, hash_name):
+    kern, blk = HASHES[hash_name]
+    legs = pair(("cksum", {}), (hash_name, {"block_" + hash_name: True}), block_checksums=True)
+
+    def sha_keyed(s):
+        return R.as_sha(O, s, hash_name, threads=NTH)
+
+    v = resident(a, "verify", sha_keyed(synth(a.verify_gib, O.PAYLOAD_PCG)), legs, (kern,))
+    v["hashed_bytes_per_step"] = v["block_stats"][hash_name] * (RECSIZE + blk)
+    if v.get(kern + "_ms_per_step"):
+        v[kern + "_gbps"] = v["hashed_bytes_per_step"] / (v[kern + "_ms_per_step"] * 1e6)
+    res = {"verify": v, "host": {}}
+    for rs in (RECSIZE, 1 << 20):
+        res["host"]["recsize_%d" % rs] = host(a, "verify", sha_keyed(synth(a.host_gib, O.PAYLOAD_PCG, rs)), legs)
+    c = R.as_send_c(O, sha_keyed(keyed(O, synth(a.recompress_gib, O.PAYLOAD_PGPAGE), NTH, R.DC_LZ4)))
+    res["recompress"] = resident(a, "recompress", c, legs, (kern,))
+    return res
+
+
+def frame_legs(a, legs, codec, kernels):
+    """resident VERIFY, host VERIFY and the ring API over pg-page records keyed for `codec`"""
+    def stream(gib, rs=RECSIZE):
+        return keyed(O, synth(gib, O.PAYLOAD_PGPAGE, rs), NTH, codec)
+
+    res = {"verify": resident(a, "verify", stream(a.verify_gib), legs, kernels, counters=tuple(legs)), "host": {}}
+    for rs in (RECSIZE, 1 << 20):
+        s = stream(a.host_gib, rs)
+        for bb in (32 << 20, 256 << 20):
+            r = host(a, "verify", s, {name: dict(kw, batch_bytes=bb) for name, kw in legs.items()})
+            res["host"]["recsize_%d_batch_%dMiB" % (rs, bb >> 20)] = dict(r, batch_bytes=bb)
+        del s
+    res["ring"] = ring(a, stream(a.ring_gib), legs)
+    return res
+
+
+def block_frames(a):
+    return frame_legs(a, pair(("cksum", {}), ("frames", {"block_frames": True}), block_checksums=True), R.DC_LZ4,
+                      ("k3_lz4_encode", "k_frame_sums", "k_frame_plan"))
+
+
+def block_lzjb(a):
+    # the flag leg keeps block_frames' leg name, "frames"
+    legs = pair(("cksum", {}), ("frames", {"block_lzjb": True}), block_checksums=True)
+    kernels = ("k_lzjb_encode", "k_zle_encode", "k_frame_sums", "k_frame_plan")
+    res = frame_legs(a, legs, R.DC_LZJB, kernels)
+    zle = keyed(O, synth(a.zle_gib, O.PAYLOAD_PGPAGE), NTH, R.DC_ZLE)
+    res["zle"] = resident(a, "verify", zle, legs, kernels, counters=tuple(legs))
+    return res
+
+
+def block_logical(a):
+    import numpy as np
+    from manatee_b200 import index_host
+    kernels = ("k_logical_plan", "k_lzjb_encode", "k_zle_encode", "k_frame_sums", "k_block_check", "k_block_sha256",
+               "k3_lz4_encode", "k2_lz4_decode")
+
+    def with_flags(**shared):
+        return pair(("base", {}), ("logical", {"block_logical": True}), block_checksums=True, **shared)
+
+    def run(mode, s, legs):
+        r = resident(a, mode, s, legs, kernels, counters=tuple(legs))
+        return dict(r, logical_bytes=int(index_host(s)[0]["lsize"].sum()))
+
+    lzjb = with_flags(block_lzjb=True)
+    res = {}
+    for gib in (a.gib, a.large_gib):
+        s = keyed(O, synth(gib, O.PAYLOAD_PGPAGE), NTH, R.DC_LZJB)
+        res["compress_lzjb_%gGiB" % gib] = run("compress", s, lzjb)
+        res["decompress_lzjb_%gGiB" % gib] = run("decompress", R.send_c_form(O, s), lzjb)
+        del s
+    x = np.ascontiguousarray(synth(a.gib, O.PAYLOAD_PGPAGE))
+    res["recompress_raw_keys_fletcher4"] = run("recompress", R.send_c_form(O, x), with_flags())
+    x = R.as_sha(O, x, "sha256", NTH)
+    res["recompress_raw_keys_sha256"] = run("recompress", R.send_c_form(O, x), with_flags(block_sha256=True))
+    del x
+    s = keyed(O, synth(a.host_gib, O.PAYLOAD_PGPAGE), NTH, R.DC_LZJB)
+    res["host_compress_lzjb"] = host(a, "compress", s, lzjb)
+    return res
+
+
+def lz4hc(a):
+    # the two encoders write different frames by design: no outputs_equal, the wire bytes of each instead
+    # (payload frames + headers; the host legs' with their wire preambles)
+    legs = pair(("zfs", {}), ("hc", {"lz4_hc": True}))
+
+    def wire(name, ob, nbytes):
+        return {name + "_wire_bytes": int(ob), name + "_ratio": nbytes / ob}
+
+    res = {"payload": "pg-page 128 KiB records (oracle.gen_payload(PAYLOAD_PGPAGE, r, 131072))"}
+    s = synth(a.gib, O.PAYLOAD_PGPAGE)
+    res["resident_compress_%gGiB" % a.gib] = resident(
+        a, "compress", s, legs, ("k3h_lz4hc_encode", "k3_lz4_encode"), counters=(), rate="input_gbps",
+        same_output=False,
+        fields=lambda name, g, ob: dict(wire(name, ob, s.size), **{name + "_lz4_encoded": g.stats()["lz4_encoded"]}))
+    h = synth(a.host_gib, O.PAYLOAD_PGPAGE)
+    res["host_compress_%gGiB" % a.host_gib] = host(a, "compress", h, legs, counters=(), rate="input_gbps",
+                                                   fields=lambda name, g, ob: wire(name, ob, h.size))
+    return res
+
+
+SHA_OPTIONS = dict(verify_gib=16.0, host_gib=2.0, recompress_gib=1.0, steps=10, warmup=2, host_steps=4,
+                   profile_steps=3)
+FRAME_OPTIONS = dict(verify_gib=16.0, host_gib=2.0, ring_gib=8.0, steps=10, warmup=2, host_steps=4, ring_steps=3,
+                     profile_steps=3)
+# subcommand -> (workload, its options and their defaults)
+WORKLOADS = {
+    "block_cksum": (block_cksum, dict(verify_gib=16.0, recompress_gib=1.0, steps=10, warmup=2)),
+    "block_sha256": (partial(block_sha, hash_name="sha256"), SHA_OPTIONS),
+    "block_sha512": (partial(block_sha, hash_name="sha512"), SHA_OPTIONS),
+    "block_frames": (block_frames, FRAME_OPTIONS),
+    "block_lzjb": (block_lzjb, dict(FRAME_OPTIONS, zle_gib=4.0)),
+    "block_logical": (block_logical, dict(gib=1.0, large_gib=4.0, host_gib=2.0, steps=10, warmup=2, host_steps=4,
+                                          profile_steps=3)),
+    "lz4hc": (lz4hc, dict(gib=1.0, host_gib=1.0, steps=5, warmup=1, host_steps=3, profile_steps=2)),
+}
+
+
+def parse_args(argv=None):
+    ap = argparse.ArgumentParser(description="cost of a GpuSnapshotStage flag on the GPU")
+    sub = ap.add_subparsers(dest="workload", required=True)
+    for name, (_, options) in WORKLOADS.items():
+        sp = sub.add_parser(name)
+        for k, v in options.items():
+            sp.add_argument("--" + k.replace("_", "-"), type=type(v), default=v)
+        sp.add_argument("--out", default=None)
+    return ap.parse_args(argv)
+
+
+def main(argv=None):
+    a = parse_args(argv)
+    import torch
+    if not torch.cuda.is_available():
+        sys.exit("flag_cost.py %s measures device time: it needs a GPU" % a.workload)
+    O.build()
+    result = {"tool": a.workload + "_cost", **gpu_info(), "steps": a.steps, "warmup": a.warmup,
+              **WORKLOADS[a.workload][0](a)}
+    line = json.dumps(result)
+    print(line)
+    if a.out:
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        with open(a.out, "w") as f:
+            f.write(line + "\n")
+
+
+if __name__ == "__main__":
+    main()
