@@ -51,6 +51,34 @@ int32_t emu_zfs_lz4_decode(const uint8_t *src, uint32_t psize, uint8_t *dst, uin
 	return out[0];
 }
 
+// RECOMPRESS's certificate of one record, launched as the pipeline launches it: k2_lz4_decode of the
+// frame with the parse by-product, then k3c_lz4_certify<flavour == 2> over `data` (lsize bytes: K2's
+// output in the product) -- flavour 0 = TabU16, 1 = TabU32, 2 = Tab17 (a compact launch).
+// 1 certified, 0 not, -1 flavour not one the product uses for lsize, -2 the frame does not decode,
+// -3 it decodes to other bytes than `data`, -4 the certified frame length is not 4 + clen.
+int32_t emu_lz4_certify(const uint8_t *frame, uint32_t psize, const uint8_t *data, uint32_t lsize, int flavour)
+{
+	using namespace mtz;
+	const bool small = lsize < (uint32_t)LZ4_64KLIMIT;
+	if ((flavour == 0) != small || flavour < 0 || flavour > 2 || (flavour == 2 && lsize > 131072u)) return -1;
+	std::vector<uint8_t> dec(lsize + 64, 0xC3);
+	std::vector<uint64_t> seqs(lsize / 8u + 1u, 0x0123456789abcdefull);   // the encoder's (unused) frame slot
+	mtz_job jd, je;
+	memset(&jd, 0, sizeof jd); memset(&je, 0, sizeof je);
+	jd.src_off = (uint64_t)(uintptr_t)frame; jd.dst_off = (uint64_t)(uintptr_t)dec.data();
+	jd.src_len = psize; jd.lsize = lsize;
+	je.src_off = (uint64_t)(uintptr_t)data; je.dst_off = (uint64_t)(uintptr_t)seqs.data(); je.lsize = lsize;
+	uint32_t seq_n = 0x5a5a5a5au, cert = 0xa5a5a5a5u;
+	emu::launch(1, LZ4_THREADS, [&] { k2_lz4_decode(nullptr, nullptr, &jd, 1, &je, &seq_n); });
+	if (jd.status != MTZ_OK) return -2;
+	if (memcmp(dec.data(), data, lsize) != 0) return -3;
+	if (flavour == 2) emu::launch(1, K3_THREADS, [&] { k3c_lz4_certify<true>(&jd, &je, &seq_n, &cert, 1); });
+	else emu::launch(1, K3_THREADS, [&] { k3c_lz4_certify<false>(&jd, &je, &seq_n, &cert, 1); });
+	if (cert == 0u) return 0;
+	const uint32_t clen = ((uint32_t)frame[0] << 24) | ((uint32_t)frame[1] << 16) | ((uint32_t)frame[2] << 8) | frame[3];
+	return cert == clen + 4u ? 1 : -4;
+}
+
 } // extern "C"
 
 // ---- guard-page buffers: [p, p+size+slack) is accessible and the next byte is not, so a

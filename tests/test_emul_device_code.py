@@ -14,6 +14,8 @@ import subprocess
 import numpy as np
 import pytest
 
+import lz4_payloads as P
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EMUL = os.path.join(ROOT, "tests", "emul")
 ECODEC = -6
@@ -40,6 +42,8 @@ def bind(so):
     L.emu_lz4_encode_block.restype = u32
     L.emu_zfs_lz4_decode.argtypes = [vp, u32, vp, u32]
     L.emu_zfs_lz4_decode.restype = C.c_int32
+    L.emu_lz4_certify.argtypes = [vp, u32, vp, u32, i32]
+    L.emu_lz4_certify.restype = C.c_int32
     L.emu_k1.argtypes = [vp, vp, u32, vp, u32, i32, u32]
     L.emu_k1.restype = C.c_int32
     L.emu_recsums_size.restype = u32
@@ -82,28 +86,9 @@ class Guarded(object):
 
 
 def _inputs(oracle, rng, n):
-    kind = int(rng.integers(0, 7))
-    if kind == 0:
-        return oracle.gen_payload(oracle.PAYLOAD_PGPAGE, int(rng.integers(0, 1 << 20)), n)
-    if kind == 1:
-        return rng.integers(0, 256, n, dtype=np.uint8)                         # incompressible
-    if kind == 2:
-        return np.zeros(n, dtype=np.uint8)
-    if kind == 3:
-        period = int(rng.integers(1, 70))
-        return np.tile(rng.integers(0, 256, period, dtype=np.uint8), n // period + 1)[:n].copy()
-    if kind == 4:
-        return rng.integers(0, int(rng.integers(2, 6)), n, dtype=np.uint8)     # tiny alphabet: hash clashes
-    if kind == 5:                                                               # far matches: >64 KiB apart
-        a = rng.integers(0, 256, n, dtype=np.uint8)
-        if n > 70000:
-            a[-3000:] = a[:3000]
-            a[66000:67000] = a[100:1100]
-        return a
-    a = oracle.gen_payload(oracle.PAYLOAD_PGPAGE, int(rng.integers(0, 1 << 20)), n).copy()
-    cut = int(rng.integers(0, n))
-    a[cut:] = rng.integers(0, 256, n - cut, dtype=np.uint8)
-    return a
+    """one payload of a family of tests/lz4_payloads.py (random, zeros, periodic, tiny alphabet, far
+    repeats, mixtures, ...), picked and seeded by rng"""
+    return P.payload(P.FAMILIES[int(rng.integers(len(P.FAMILIES)))], int(rng.integers(0, 1 << 20)), n)
 
 
 def test_k3_encoder_source_is_bit_exact_on_the_cpu(emu, oracle):
