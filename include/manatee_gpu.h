@@ -38,7 +38,8 @@ extern "C" {
 #define MTZ_ECUDA    -3   /* CUDA runtime failure, see mtz_last_error */
 #define MTZ_EFORMAT  -4   /* malformed send stream (bad magic / type / length) */
 #define MTZ_ECKSUM   -5   /* embedded or END Fletcher-4 mismatch (like zfs recv ECKSUM) */
-#define MTZ_ECODEC   -6   /* LZ4 frame does not decode to drr_logical_size */
+#define MTZ_ECODEC   -6   /* LZ4 frame does not decode to drr_logical_size (MTZ_FLAG_COMPRESSED_IN: an
+                           * lzjb / zle frame, or a compression the stage has no decoder for) */
 #define MTZ_ENOSPC   -7   /* output capacity exceeded */
 #define MTZ_ENOMEM   -8
 #define MTZ_EOF      -9   /* consumer: stream finished and fully drained */
@@ -130,6 +131,24 @@ extern "C" {
                                   * DECOMPRESS, RECOMPRESS and PASSTHROUGH accept the flag and do not
                                   * change */
 
+#define MTZ_FLAG_COMPRESSED_IN 512u /* COMPRESS: accept a `zfs send -c` stream (DRR_BEGIN with the COMPRESSED
+                                  * feature; without this flag MTZ_EINVAL).  By drr_compressiontype: 0 is
+                                  * encoded as always; LZ4 (15) is forwarded byte for byte, header and
+                                  * payload, with only the stream checksum re-stamped (also under
+                                  * MTZ_FLAG_LZ4_HC); lzjb (3) and zle (14) are decoded on the GPU, ZFS's
+                                  * lzjb_decompress / zle_decompress bounded by the payload, then stored LZ4
+                                  * or raw like a raw record; any other compression (gzip, zstd, unknown),
+                                  * and a frame that does not decode to drr_logical_size, fails the handle
+                                  * with MTZ_ECODEC at that record.  The wire stays lz4-stage-v1: any
+                                  * DECOMPRESS stage decodes it into exactly the stream `zfs send` without -c
+                                  * would have produced.  With MTZ_FLAG_BLOCK_CKSUM a record that arrives as
+                                  * its disk frame is compared as it is, as in VERIFY (lzjb / zle with
+                                  * MTZ_FLAG_BLOCK_LZJB), before MTZ_FLAG_BLOCK_LOGICAL's rules; the
+                                  * receiver's block counters may then differ from the sender's, since it
+                                  * sees LZ4 or raw where the sender saw the disk frame.  Counters:
+                                  * mtz_get_compressed_in_stats.  VERIFY, DECOMPRESS, RECOMPRESS and
+                                  * PASSTHROUGH accept the flag and do not change */
+
 typedef struct mtz_handle mtz_handle;
 
 #define MTZ_MAX_DEVICES 16
@@ -199,6 +218,16 @@ typedef struct mtz_block_stats {
 	uint64_t logical_checked;   /* MTZ_FLAG_BLOCK_LOGICAL: records compared thanks to that flag (also counted
 	                               in logical_ok / frame_ok / frame_miss, or the cause of the failure) */
 } mtz_block_stats;
+
+/* MTZ_FLAG_COMPRESSED_IN counters (all zero without the flag).  mtz_stats.lz4_encoded keeps counting
+ * the frames the stage encoded, mtz_stats.lz4_decoded the LZ4 frames it decoded: neither counts these. */
+typedef struct mtz_compressed_in_stats {
+	uint32_t struct_size;       /* sizeof(mtz_compressed_in_stats), set by the caller */
+	uint32_t pad;
+	uint64_t lz4_passed;        /* DRR_WRITEs that arrived LZ4 and were forwarded as they are */
+	uint64_t lzjb_decoded;      /* ... that arrived lzjb and were decoded on the GPU */
+	uint64_t zle_decoded;       /* ... that arrived zle and were decoded on the GPU */
+} mtz_compressed_in_stats;
 
 /* One DRR record as seen by the kernels (32 B, little endian). */
 typedef struct mtz_rec {
@@ -276,6 +305,8 @@ int32_t mtz_cancel(mtz_handle *h);
 int32_t mtz_get_stats(mtz_handle *h, mtz_stats *st);
 /* fills min(st->struct_size, sizeof(mtz_block_stats)) bytes */
 int32_t mtz_get_block_stats(mtz_handle *h, mtz_block_stats *st);
+/* fills min(st->struct_size, sizeof(mtz_compressed_in_stats)) bytes */
+int32_t mtz_get_compressed_in_stats(mtz_handle *h, mtz_compressed_in_stats *st);
 /* running Fletcher-4 of the OUTPUT stream before DRR_END (== drr_end.drr_checksum) */
 int32_t mtz_end_checksum(mtz_handle *h, uint64_t out[4]);
 

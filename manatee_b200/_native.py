@@ -24,6 +24,7 @@ FLAG_BLOCK_FRAMES = 32
 FLAG_BLOCK_LZJB = 64
 FLAG_BLOCK_LOGICAL = 128
 FLAG_LZ4_HC = 256
+FLAG_COMPRESSED_IN = 512
 XCHG_FIRST, XCHG_LAST = 1, 2
 MODE_NAMES = {"verify": 0, "compress": 1, "decompress": 2, "recompress": 3, "passthrough": 4}
 
@@ -66,6 +67,14 @@ class BlockStats(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_[2:]}
 
 
+class CompressedInStats(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("pad", C.c_uint32), ("lz4_passed", C.c_uint64),
+                ("lzjb_decoded", C.c_uint64), ("zle_decoded", C.c_uint64)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_[2:]}
+
+
 class Rec(C.Structure):
     _fields_ = [("off", C.c_uint64), ("payload", C.c_uint32), ("type", C.c_uint32),
                 ("lsize", C.c_uint32), ("comp", C.c_uint32), ("resv", C.c_uint64)]
@@ -76,7 +85,7 @@ SYMBOLS = [
     "mtz_abi_version", "mtz_device_count", "mtz_open", "mtz_close", "mtz_last_error",
     "mtz_strerror", "mtz_ring_acquire", "mtz_ring_commit", "mtz_write", "mtz_flush",
     "mtz_out_peek", "mtz_out_consume", "mtz_read", "mtz_event_fd", "mtz_get_stats",
-    "mtz_get_block_stats", "mtz_end_checksum", "mtz_host_alloc", "mtz_host_free", "mtz_process_host",
+    "mtz_get_block_stats", "mtz_get_compressed_in_stats", "mtz_end_checksum", "mtz_host_alloc", "mtz_host_free", "mtz_process_host",
     "mtz_index_host", "mtz_dev_index", "mtz_dev_submit", "mtz_dev_aggregate",
     "mtz_dev_finish", "mtz_dev_reset", "mtz_dev_aggregate_async", "mtz_dev_finish_gathered", "mtz_set_carry",
     "mtz_k_lz4_decode", "mtz_k_lz4_encode", "mtz_k_lz4hc_encode",
@@ -129,6 +138,7 @@ def lib():
     L.mtz_event_fd.argtypes = [H]
     L.mtz_get_stats.argtypes = [H, C.POINTER(Stats)]
     L.mtz_get_block_stats.argtypes = [H, C.POINTER(BlockStats)]
+    L.mtz_get_compressed_in_stats.argtypes = [H, C.POINTER(CompressedInStats)]
     L.mtz_end_checksum.argtypes = [H, C.POINTER(u64 * 4)]
     L.mtz_host_alloc.argtypes = [sz, C.POINTER(vp)]
     L.mtz_host_free.argtypes = [vp]

@@ -30,6 +30,8 @@ namespace mtz {
                                // RECOMPRESS lzjb / zle records that arrive as their disk frame
 #define BLK_FR_LOGICAL 4u      // MTZ_FLAG_BLOCK_LOGICAL: the re-encoding modes check keys from the logical
                                // bytes they hold (k_logical_plan, kernels_frames.cuh)
+#define BLK_FR_CIN     8u      // COMPRESS with MTZ_FLAG_COMPRESSED_IN: with BLK_FR_LZJB, lzjb / zle records that
+                               // arrive as their disk frame are compared as they are, as in VERIFY
 // BlockClass.src: where the bytes a key is compared with are
 #define BLK_SRC_IN     0       // the input payload
 #define BLK_SRC_OUT    1       // the output payload of a re-encoding mode
@@ -70,7 +72,8 @@ __host__ __device__ __forceinline__ Ck4 strip_head8(const Ck4 &whole, const Ck4 
 // `have_out` = the output records of a re-encoding mode are at hand; `frames` = BLK_FR_* bits: with
 // BLK_FR_LZ4 (VERIFY with MTZ_FLAG_BLOCK_FRAMES) the encoder's LZ4 frames of the raw records are, with
 // BLK_FR_LZJB (MTZ_FLAG_BLOCK_LZJB) lzjb and zle keys are checked: against the input payload when
-// the record arrives as that frame (VERIFY, RECOMPRESS: passed through), in VERIFY against the
+// the record arrives as that frame (VERIFY, RECOMPRESS: passed through; COMPRESS with BLK_FR_CIN: before
+// it is decoded), in VERIFY against the
 // encoder's frame of a raw record.  With BLK_FR_LOGICAL the re-encoding modes also use the logical
 // bytes they hold (the raw input payload, or in DECOMPRESS and RECOMPRESS K2's output for a record that
 // arrives LZ4; COMPRESS decodes nothing, so an LZ4 record it is handed stays skipped), rows marked
@@ -110,7 +113,9 @@ __device__ __forceinline__ BlockClass block_classify(const uint8_t *hdr, const m
 			else if (raw_in && (frames & BLK_FR_LZ4) && mode == MTZ_MODE_VERIFY) { c.what = 2; c.src = BLK_SRC_JOB; }
 			else if (raw_in && mode == MTZ_MODE_DECOMPRESS && logical) { c.what = 2; c.src = BLK_SRC_NONE; c.logical = true; }
 		} else if ((frames & BLK_FR_LZJB) && (dc == BLK_DC_LZJB || dc == BLK_DC_ZLE)) {
-			if (rec.comp == dc && (mode == MTZ_MODE_VERIFY || mode == MTZ_MODE_RECOMPRESS)) { c.what = 2; c.src = BLK_SRC_IN; }
+			if (rec.comp == dc && (mode == MTZ_MODE_VERIFY || mode == MTZ_MODE_RECOMPRESS || (frames & BLK_FR_CIN))) {
+				c.what = 2; c.src = BLK_SRC_IN;
+			}
 			else if (raw_in && mode == MTZ_MODE_VERIFY) { c.what = 2; c.src = BLK_SRC_JOB; }
 			else if ((raw_in || lz4_in) && logical) { c.what = 2; c.src = BLK_SRC_JOB; c.logical = true; }
 		}

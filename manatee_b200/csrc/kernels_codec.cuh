@@ -14,12 +14,16 @@
 
 namespace mtz {
 
-#define CF_DEC    1u      // payload is a ZFS-LZ4 frame that this mode decodes
+#define CF_DEC    1u      // payload is a frame that this mode decodes: ZFS-LZ4 (K2), or in COMPRESS with
+                          // MTZ_FLAG_COMPRESSED_IN lzjb / zle (k_lzjb_decode / k_zle_decode)
 #define CF_ENC    2u      // (decoded or raw) logical payload is offered to the encoder
 #define CF_WRITE  4u
+#define CF_PASS   8u      // COMPRESS with MTZ_FLAG_COMPRESSED_IN: an LZ4 frame forwarded as it is
+#define CF_BAD    16u     // ... a compression the stage cannot decode: its decode job fails
 
 #define FEAT_LZ4        (1ull << 17)
 #define FEAT_COMPRESSED (1ull << 22)
+#define FEAT_EMBED_DATA (1ull << 16)
 // wire format "lz4-stage-v1": a 32-byte preamble in front of every DRR_BEGIN of a COMPRESS output
 // (u64 magic "MTZLZ4W1", u32 version, u32 flags, 16 zero bytes), outside the stream checksum.  The
 // host paths write and strip it; the kernels only see its one flag, carried in mtz_rec.resv of
@@ -45,11 +49,20 @@ struct CodecResult {       // device, mirrored to pinned host
 	uint32_t n_dec;        // records decoded
 	uint32_t n_enc;        // records stored compressed on output
 	uint32_t n_cert;       // ... of which certified (input frame == encoder output), not re-encoded
+	uint32_t n_pass;       // COMPRESS with MTZ_FLAG_COMPRESSED_IN: LZ4 records forwarded as they are
+	uint32_t n_lzjb;       // ... lzjb records decoded (not counted in n_dec)
+	uint32_t n_zle;        // ... zle records decoded (likewise)
+	uint32_t pad;
 };
 
 // ---- plan, step 1: flags + scratch need -----------------------------------
+// `cin`: COMPRESS with MTZ_FLAG_COMPRESSED_IN.  The one place that decides what becomes of a
+// compressed DRR_WRITE there: lzjb / zle are decoded and offered to the encoder like a raw record,
+// LZ4 is forwarded as it is, any other compression fails the record (MTZ_ECODEC).
+#define ZIO_LZJB 3u
+#define ZIO_ZLE  14u
 __global__ void k_plan_need(const mtz_rec *__restrict__ recs, uint32_t n, uint32_t mode,
-    CodecRec *__restrict__ cr, uint64_t *__restrict__ vals)
+    CodecRec *__restrict__ cr, uint64_t *__restrict__ vals, bool cin = false)
 {
 	const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
 	if (r >= n) return;
@@ -59,6 +72,8 @@ __global__ void k_plan_need(const mtz_rec *__restrict__ recs, uint32_t n, uint32
 		f |= CF_WRITE;
 		if (rec.comp == ZIO_LZ4 && (mode == MTZ_MODE_DECOMPRESS || mode == MTZ_MODE_RECOMPRESS))
 			f |= CF_DEC;
+		if (cin && mode == MTZ_MODE_COMPRESS && rec.comp != 0u)
+			f |= rec.comp == ZIO_LZJB || rec.comp == ZIO_ZLE ? CF_DEC : rec.comp == ZIO_LZ4 ? CF_PASS : CF_BAD;
 		if ((mode == MTZ_MODE_COMPRESS || mode == MTZ_MODE_RECOMPRESS) &&
 		    (rec.comp == 0u || (f & CF_DEC)))
 			f |= CF_ENC;
@@ -127,7 +142,9 @@ __global__ void k_plan_jobs(const uint8_t *__restrict__ d_in, const mtz_rec *__r
 	mtz_job jd, je;
 	jd.src_off = jd.dst_off = 0; jd.src_len = 0; jd.lsize = 0; jd.out_len = 0; jd.status = 0;
 	je = jd;
-	if (c.flags & CF_DEC) {
+	if (c.flags & CF_BAD) {
+		jd.status = MTZ_ECODEC;                 // no decoder for it
+	} else if (c.flags & CF_DEC) {
 		jd.src_off = (uint64_t)(uintptr_t)pay;
 		jd.dst_off = (uint64_t)(uintptr_t)(d_logical + c.scratch);
 		jd.src_len = rec.payload; jd.lsize = rec.lsize;
@@ -152,11 +169,13 @@ __global__ void k_layout(const mtz_rec *__restrict__ recs, uint32_t n, CodecRec 
 	const mtz_rec rec = recs[r];
 	CodecRec c = cr[r];
 	uint32_t len = rec.payload;
+	if (c.flags & CF_BAD) atomicMin(&res->bad, r + rec_base);      // stays as it is: the batch fails
 	if (c.flags & CF_DEC) {
 		if (dec[r].status != MTZ_OK) atomicMin(&res->bad, r + rec_base);
-		else atomicAdd(&res->n_dec, 1u);
+		else atomicAdd(rec.comp == ZIO_LZJB ? &res->n_lzjb : rec.comp == ZIO_ZLE ? &res->n_zle : &res->n_dec, 1u);
 		len = rec.lsize;
 	}
+	if (c.flags & CF_PASS) atomicAdd(&res->n_pass, 1u);
 	if ((c.flags & CF_ENC) && enc[r].out_len < rec.lsize) {
 		len = enc[r].out_len;
 		atomicAdd(&res->n_enc, 1u);

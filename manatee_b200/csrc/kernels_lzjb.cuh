@@ -10,6 +10,13 @@
 // already apply to K3's frames.  A frame never exceeds d_len < lsize: the slots stay disjoint.
 //   k_lzjb_encode  one warp per job, the 1024 x u16 lempel table in shared memory (2 KiB per warp)
 //   k_zle_encode   one warp per job, zero and literal runs found by ballot
+// COMPRESS with MTZ_FLAG_COMPRESSED_IN decodes the lzjb and zle records of a `zfs send -c` stream
+// before K3 sees them, with the decoders restated from the same files:
+//   k_lzjb_decode  one warp per job, 32 items per round, the output window in shared memory (4 KiB per warp)
+//   k_zle_decode   one warp per job, a walk of the length tokens with warp-wide copies and zero fills
+// Both keep K2's access contract (include/manatee_gpu.h): read only [src, src+src_len), write only
+// [dst, dst+lsize).  ZFS's lzjb loop does not bound its source; these do, and a frame whose decode
+// would read at or past the end of its payload is MTZ_ECODEC like a frame ZFS rejects.
 #pragma once
 #include "kernels_block.cuh"
 
@@ -212,6 +219,152 @@ k_zle_encode(mtz_job *__restrict__ jobs, uint32_t njobs)
 		const uint32_t ps = zio_sector_pad(dst, c, job.lsize, lane);
 		__syncwarp();
 		if (lane == 0) { jobs[j].out_len = ps; jobs[j].status = MTZ_OK; }
+	}
+}
+
+// ---- decoders -----------------------------------------------------------------------------------
+#define LZJB_RING 4096u             // output window per warp: 1023 bytes of history + a round's <= 32 x 66
+
+// lzjb_decompress(src, dst, s_len, lsize): a copymap byte, then 8 items, 1 byte per literal and 2 per
+// match (bit set: length (b0 >> 2) + 3, offset ((b0 << 8) | b1) & 1023).  A copymap byte fixes where
+// its 8 items start, so a round takes 4 copymap bytes and 32 items, one per lane, from a 96-byte source
+// window held in registers (a round reads at most 4 + 64 bytes).  One shuffle scan of the item lengths
+// places every output; literals are stored in parallel, matches resolved in item order (a match reads
+// only output before its own, so a periodic copy covers an offset below the length).  The output is
+// built in a shared-memory ring and streamed to dst in whole words behind the decode.
+// A needed item past the end of the source, an offset of 0 (ZFS would copy destination bytes it never
+// wrote) or one reaching before dst is MTZ_ECODEC; items past lsize are not read, like the C loop's.
+__device__ __forceinline__ int32_t warp_lzjb_decode(const uint8_t *__restrict__ src, uint32_t s_len,
+    uint8_t *__restrict__ dst, uint32_t lsize, uint8_t *ring, int lane)
+{
+	const uint32_t FULL = 0xffffffffu, RMASK = LZJB_RING - 1u;
+	const bool wide = ((uintptr_t)dst & 3u) == 0u;
+	const uint32_t g = (uint32_t)lane >> 3, b = (uint32_t)lane & 7u;
+	uint32_t ip = 0, op = 0, fl = 0;        // next copymap byte, bytes decoded, bytes stored to dst
+	while (op < lsize) {
+		uint32_t win = 0;                   // source byte ip + k sits in lane k & 31, byte k >> 5
+#pragma unroll
+		for (uint32_t k = 0; k < 3u; k++) {
+			const uint32_t q = ip + 32u * k + (uint32_t)lane;
+			if (q < s_len) win |= (uint32_t)src[q] << (8u * k);
+		}
+		auto byte_at = [&](uint32_t r) -> uint32_t {
+			return (__shfl_sync(FULL, win, (int)(r & 31u)) >> (8u * (r >> 5))) & 0xffu;
+		};
+		// the 4 copymap bytes of the round and where they sit (relative to ip)
+		const uint32_t q0 = 0u, c0 = byte_at(q0);
+		const uint32_t q1 = q0 + 9u + (uint32_t)__popc(c0), c1 = byte_at(q1);
+		const uint32_t q2 = q1 + 9u + (uint32_t)__popc(c1), c2 = byte_at(q2);
+		const uint32_t q3 = q2 + 9u + (uint32_t)__popc(c2), c3 = byte_at(q3);
+		const uint32_t cm = g == 0u ? c0 : g == 1u ? c1 : g == 2u ? c2 : c3;
+		const uint32_t qg = g == 0u ? q0 : g == 1u ? q1 : g == 2u ? q2 : q3;
+		const bool ism = (cm >> b) & 1u;
+		const uint32_t r = qg + 1u + b + (uint32_t)__popc(cm & ((1u << b) - 1u));
+		const uint32_t b0 = byte_at(r), b1 = byte_at(r + 1u);
+		const uint32_t len = ism ? (b0 >> 2) + LZJB_MATCH_MIN : 1u;
+		const uint32_t off = ((b0 << 8) | b1) & LZJB_OFFSET_MASK;
+		uint32_t inc = len;
+#pragma unroll
+		for (int d = 1; d < 32; d <<= 1) {
+			const uint32_t up = __shfl_up_sync(FULL, inc, d);
+			if (lane >= d) inc += up;
+		}
+		const uint32_t o = op + inc - len;
+		const bool need = o < lsize;
+		const bool bad = need && (ip + qg >= s_len || ip + r + (ism ? 2u : 1u) > s_len ||
+		    (ism && (off == 0u || off > o)));
+		if (__any_sync(FULL, bad)) return MTZ_ECODEC;
+		const uint32_t clen = need ? min(len, lsize - o) : 0u;
+		if (need && !ism) ring[o & RMASK] = (uint8_t)b0;
+		__syncwarp();
+		for (uint32_t mm = __ballot_sync(FULL, need && ism); mm != 0u; mm &= mm - 1u) {
+			const int k = __ffs(mm) - 1;
+			const uint32_t mo = __shfl_sync(FULL, o, k), moff = __shfl_sync(FULL, off, k);
+			const uint32_t ml = __shfl_sync(FULL, clen, k);
+			for (uint32_t i = (uint32_t)lane; i < ml; i += 32u)
+				ring[(mo + i) & RMASK] = ring[(mo - moff + (moff < ml ? i % moff : i)) & RMASK];
+			__syncwarp();
+		}
+		const uint32_t total = __shfl_sync(FULL, inc, 31);
+		if (op + total >= lsize) {
+			op = lsize;
+		} else {
+			op += total;
+			ip += q3 + 9u + (uint32_t)__popc(c3);
+		}
+		// everything decoded so far up to a word boundary (all of it at the end) goes to dst
+		const uint32_t fe = op == lsize ? lsize : (op & ~3u);
+		if (wide) {
+			const uint32_t fw = fe & ~3u;
+			for (uint32_t w = fl + 4u * (uint32_t)lane; w < fw; w += 128u)
+				*reinterpret_cast<uint32_t *>(dst + w) = *reinterpret_cast<const uint32_t *>(ring + (w & RMASK));
+			for (uint32_t i = fw + (uint32_t)lane; i < fe; i += 32u) dst[i] = ring[i & RMASK];
+			fl = fw;
+		} else {
+			for (uint32_t i = fl + (uint32_t)lane; i < fe; i += 32u) dst[i] = ring[i & RMASK];
+			fl = fe;
+		}
+		__syncwarp();
+	}
+	return MTZ_OK;
+}
+
+// zle_decompress(src, dst, s_len, lsize, 64): a length byte n - 1; n <= 64 is a literal run of n bytes,
+// otherwise a run of n - 64 zeros.  A run past either end, or a source that ends before lsize bytes,
+// is MTZ_ECODEC.  Every decision is warp-uniform.
+__device__ __forceinline__ int32_t warp_zle_decode(const uint8_t *__restrict__ src, uint32_t s_len,
+    uint8_t *__restrict__ dst, uint32_t lsize, int lane)
+{
+	uint32_t sp = 0, dp = 0;
+	while (sp < s_len && dp < lsize) {
+		uint32_t n = 1u + src[sp++];
+		if (n <= ZLE_N) {
+			if (sp + n > s_len || dp + n > lsize) return MTZ_ECODEC;
+			for (uint32_t i = (uint32_t)lane; i < n; i += 32u) dst[dp + i] = src[sp + i];
+			sp += n;
+		} else {
+			n -= ZLE_N;
+			if (dp + n > lsize) return MTZ_ECODEC;
+			for (uint32_t i = (uint32_t)lane; i < n; i += 32u) dst[dp + i] = 0;
+		}
+		dp += n;
+	}
+	return dp == lsize ? MTZ_OK : MTZ_ECODEC;
+}
+
+// One warp per job (grid-stride) of a record whose drr_compressiontype is lzjb: the frame
+// [src_off, src_off + src_len) decoded to the lsize bytes at dst_off, status MTZ_OK or MTZ_ECODEC.
+// Jobs of other records, and empty jobs (lsize 0), are left alone.  `recs` indexes like `jobs`.
+__global__ void __launch_bounds__(LZJB_THREADS)
+k_lzjb_decode(const mtz_rec *__restrict__ recs, mtz_job *__restrict__ jobs, uint32_t njobs)
+{
+	__shared__ uint32_t s_ring[LZJB_WARPS][LZJB_RING / 4u];
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	const uint32_t gw = blockIdx.x * LZJB_WARPS + (uint32_t)warp;
+	const uint32_t nw = gridDim.x * LZJB_WARPS;
+	for (uint32_t j = gw; j < njobs; j += nw) {
+		const mtz_job job = jobs[j];
+		if (job.lsize == 0u || recs[j].comp != BLK_DC_LZJB) continue;
+		const int32_t st = warp_lzjb_decode(reinterpret_cast<const uint8_t *>((uintptr_t)job.src_off), job.src_len,
+		    reinterpret_cast<uint8_t *>((uintptr_t)job.dst_off), job.lsize,
+		    reinterpret_cast<uint8_t *>(s_ring[warp]), lane);
+		if (lane == 0) { jobs[j].status = st; jobs[j].out_len = st == MTZ_OK ? job.lsize : 0u; }
+	}
+}
+
+// Likewise for the records whose drr_compressiontype is zle.
+__global__ void __launch_bounds__(LZJB_THREADS)
+k_zle_decode(const mtz_rec *__restrict__ recs, mtz_job *__restrict__ jobs, uint32_t njobs)
+{
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	const uint32_t gw = blockIdx.x * LZJB_WARPS + (uint32_t)warp;
+	const uint32_t nw = gridDim.x * LZJB_WARPS;
+	for (uint32_t j = gw; j < njobs; j += nw) {
+		const mtz_job job = jobs[j];
+		if (job.lsize == 0u || recs[j].comp != BLK_DC_ZLE) continue;
+		const int32_t st = warp_zle_decode(reinterpret_cast<const uint8_t *>((uintptr_t)job.src_off), job.src_len,
+		    reinterpret_cast<uint8_t *>((uintptr_t)job.dst_off), job.lsize, lane);
+		if (lane == 0) { jobs[j].status = st; jobs[j].out_len = st == MTZ_OK ? job.lsize : 0u; }
 	}
 }
 

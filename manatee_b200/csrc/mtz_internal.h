@@ -189,6 +189,7 @@ struct mtz_handle {
 	const mtz_rec *dv_recs = nullptr;
 	mtz::BlockPending bpend;
 	mtz_block_stats bstats{};
+	mtz_compressed_in_stats cstats{};  // MTZ_FLAG_COMPRESSED_IN counters (under stats_mu)
 
 	mtz::IndexResult *d_ires = nullptr, *h_ires = nullptr;
 	mtz::IndexShared *d_ishared = nullptr;

@@ -473,6 +473,20 @@ int32_t mtz_get_block_stats(mtz_handle *h, mtz_block_stats *st)
 	return MTZ_OK;
 }
 
+int32_t mtz_get_compressed_in_stats(mtz_handle *h, mtz_compressed_in_stats *st)
+{
+	if (h == nullptr || st == nullptr || st->struct_size < 2 * sizeof(uint32_t)) return MTZ_EINVAL;
+	mtz_compressed_in_stats c;
+	{
+		std::lock_guard<std::mutex> g(h->stats_mu);
+		c = h->cstats;
+	}
+	const size_t n = std::min((size_t)st->struct_size, sizeof c);
+	c.struct_size = (uint32_t)n; c.pad = 0;
+	memcpy(st, &c, n);
+	return MTZ_OK;
+}
+
 int32_t mtz_end_checksum(mtz_handle *h, uint64_t out[4])
 {
 	if (h == nullptr || out == nullptr) return MTZ_EINVAL;
@@ -572,6 +586,7 @@ static bool block_frames_on(const mtz_handle *h)
 }
 static bool block_lzjb_on(const mtz_handle *h) { return (h->cfg.flags & MTZ_FLAG_BLOCK_LZJB) != 0; }
 static bool is_codec_mode(uint32_t m);
+static bool cin_on(const mtz_handle *h);
 // COMPRESS / DECOMPRESS / RECOMPRESS with MTZ_FLAG_BLOCK_LOGICAL: the block check runs jobs over the
 // logical bytes (launch_block_logical); VERIFY accepts the flag and does not change
 static bool block_logical_on(const mtz_handle *h)
@@ -584,7 +599,8 @@ static bool block_logical_on(const mtz_handle *h)
 static uint32_t block_fcodecs(const mtz_handle *h)
 {
 	return ((h->cfg.flags & MTZ_FLAG_BLOCK_FRAMES) && h->cfg.mode == MTZ_MODE_VERIFY ? BLK_FR_LZ4 : 0u) |
-	    (block_lzjb_on(h) ? BLK_FR_LZJB : 0u) | (block_logical_on(h) ? BLK_FR_LOGICAL : 0u);
+	    (block_lzjb_on(h) ? BLK_FR_LZJB : 0u) | (block_logical_on(h) ? BLK_FR_LOGICAL : 0u) |
+	    (cin_on(h) ? BLK_FR_CIN : 0u);
 }
 static uint32_t block_hashed(const mtz_handle *h)
 {
@@ -777,6 +793,14 @@ static bool lz4hc_on(const mtz_handle *h)
 	return h->cfg.mode == MTZ_MODE_COMPRESS && (h->cfg.flags & MTZ_FLAG_LZ4_HC) != 0;
 }
 
+// COMPRESS with MTZ_FLAG_COMPRESSED_IN takes `zfs send -c` streams: lzjb / zle records are decoded
+// (k_lzjb_decode / k_zle_decode) and re-encoded, LZ4 records forwarded; the other modes accept the
+// flag and do not change
+static bool cin_on(const mtz_handle *h)
+{
+	return h->cfg.mode == MTZ_MODE_COMPRESS && (h->cfg.flags & MTZ_FLAG_COMPRESSED_IN) != 0;
+}
+
 // K3h's hash tables: one per warp of its persistent grid (launch_k3h)
 static size_t hc_tab_bytes(const mtz_handle *h)
 {
@@ -795,7 +819,7 @@ static int32_t codec_alloc(mtz_handle *h, CodecBufs &cb, size_t rec_cap, size_t 
 	MTZ_CU(h, cudaMalloc(&cb.out_recs, rec_cap * sizeof(mtz_rec)));
 	MTZ_CU(h, cudaMalloc(&cb.osums, rec_cap * sizeof(RecSums)));
 	MTZ_CU(h, cudaMalloc(&cb.steps, rec_cap * sizeof(StampStep)));
-	if (h->cfg.mode == MTZ_MODE_DECOMPRESS || h->cfg.mode == MTZ_MODE_RECOMPRESS)
+	if (h->cfg.mode == MTZ_MODE_DECOMPRESS || h->cfg.mode == MTZ_MODE_RECOMPRESS || cin_on(h))
 		MTZ_CU(h, cudaMalloc(&cb.d_logical, scratch_cap + 512));
 	if (h->cfg.mode != MTZ_MODE_DECOMPRESS) MTZ_CU(h, cudaMalloc(&cb.d_enc, scratch_cap + 512));
 	if (h->cfg.mode == MTZ_MODE_VERIFY && block_lzjb_on(h) && (h->cfg.flags & MTZ_FLAG_BLOCK_FRAMES))
@@ -876,7 +900,8 @@ static int32_t codec_launch_pre(mtz_handle *h, cudaStream_t st, CodecBufs &cb, c
 	return MTZ_OK;
 }
 
-// plan + K2 (decode) of one (sub-)batch
+// plan + K2 (decode) of one (sub-)batch; in COMPRESS with MTZ_FLAG_COMPRESSED_IN the lzjb and zle
+// decoders in K2's place (every decode job of that mode is one of theirs)
 static int32_t codec_launch_dec(mtz_handle *h, cudaStream_t st, CodecBufs &cb, const uint8_t *d_in,
     const mtz_rec *d_recs, size_t nrec)
 {
@@ -884,7 +909,7 @@ static int32_t codec_launch_dec(mtz_handle *h, cudaStream_t st, CodecBufs &cb, c
 	if (nrec > cb.rec_cap) return fail(h, MTZ_ENOSPC, "codec batch of %zu records exceeds %zu", nrec, cb.rec_cap);
 	const uint32_t n = (uint32_t)nrec, mode = h->cfg.mode;
 	const unsigned tb = 256, gb = (n + tb - 1) / tb;
-	k_plan_need<<<gb, tb, 0, st>>>(d_recs, n, mode, cb.cr, cb.vals);
+	k_plan_need<<<gb, tb, 0, st>>>(d_recs, n, mode, cb.cr, cb.vals, cin_on(h));
 	k_xscan_u64<<<1, XSCAN_THREADS, 0, st>>>(cb.vals, cb.offs, n, nullptr, nullptr);
 	k_plan_jobs<<<gb, tb, 0, st>>>(d_in, d_recs, n, cb.cr, cb.offs, cb.d_logical, cb.d_enc, cb.dec, cb.enc);
 	MTZ_CU(h, cudaGetLastError());
@@ -892,6 +917,12 @@ static int32_t codec_launch_dec(mtz_handle *h, cudaStream_t st, CodecBufs &cb, c
 	if (mode != MTZ_MODE_COMPRESS) {
 		int32_t rc = launch_k2(h, st, nullptr, nullptr, cb.dec, n, cb.seq_n ? cb.enc : nullptr, cb.seq_n);
 		if (rc != MTZ_OK) return rc;
+	} else if (cin_on(h)) {
+		const unsigned gl = (unsigned)std::min<size_t>((nrec + LZJB_WARPS - 1) / LZJB_WARPS, (size_t)h->sm_count * 8);
+		k_lzjb_decode<<<gl, LZJB_THREADS, 0, st>>>(d_recs, cb.dec, n);
+		k_zle_decode<<<gl, LZJB_THREADS, 0, st>>>(d_recs, cb.dec, n);
+		MTZ_CU(h, cudaGetLastError());
+		count_launch(h, 2);
 	}
 	return MTZ_OK;
 }
@@ -979,6 +1010,7 @@ int32_t mtz_dev_reset(mtz_handle *h)
 	h->stats.bad_record = ~0ull;
 	h->bstats = mtz_block_stats();
 	if (block_on(h)) h->bstats.first_frame_miss = ~0ull;
+	h->cstats = mtz_compressed_in_stats();
 	return MTZ_OK;
 }
 
@@ -1435,13 +1467,17 @@ static int32_t dev_finish_impl(mtz_handle *h, const uint64_t carry_in[4], const 
 				std::lock_guard<std::mutex> g(h->stats_mu);
 				if (bad < h->stats.bad_record) h->stats.bad_record = bad;
 			}
-			return fail(h, MTZ_ECODEC, "LZ4 frame of record %llu does not decode to drr_logical_size",
+			return fail(h, MTZ_ECODEC, "record %llu: its frame does not decode to drr_logical_size, or no decoder "
+			    "takes its compression",
 			    (unsigned long long)bad);
 		}
 		std::lock_guard<std::mutex> g(h->stats_mu);
 		h->stats.lz4_decoded += c.n_dec;
 		h->stats.lz4_encoded += c.n_enc;
 		h->stats.lz4_certified += c.n_cert;
+		h->cstats.lz4_passed += c.n_pass;
+		h->cstats.lzjb_decoded += c.n_lzjb;
+		h->cstats.zle_decoded += c.n_zle;
 	}
 	if (out_bytes) *out_bytes = ob;
 	rc = account_result(h, r, h->dv_first, h->dv_nrec, h->dv_in_bytes, ob, block_on(h) ? &h->bpend : nullptr);
@@ -1511,6 +1547,14 @@ static int wire_parse(const uint8_t *p, uint32_t *flags)
 	return 1;
 }
 
+// The preamble's WIRE_F_ORIG_LZ4: the stream `zfs send` without -c would have produced carries the
+// LZ4 feature.  -c alone sets it whenever the pool's lz4 feature is active, without -c only -e
+// (EMBED_DATA) does ([EXTERNAL] dmu_send.c), so a compressed stream keeps it only with EMBED_DATA.
+static uint32_t wire_orig_lz4(uint64_t feat)
+{
+	return (feat & FEAT_LZ4) && (!(feat & FEAT_COMPRESSED) || (feat & FEAT_EMBED_DATA)) ? WIRE_F_ORIG_LZ4 : 0u;
+}
+
 // returns 1 accepted, 0 batch is full (cut first), <0 error (already reported)
 static int32_t batch_accept(mtz_handle *h, const Slot &s, BatchCut &bc, const uint8_t *hdr,
     int64_t pl, uint32_t ls, uint32_t comp, uint64_t stream_off, mtz_rec *out, WireState *ws)
@@ -1533,11 +1577,12 @@ static int32_t batch_accept(mtz_handle *h, const Slot &s, BatchCut &bc, const ui
 		const uint64_t vi = rd64(hdr + 16);
 		const uint64_t feat = (vi >> 2) & ((1ull << 30) - 1ull);
 		if (h->cfg.mode == MTZ_MODE_COMPRESS) {
-			if (feat & FEAT_COMPRESSED) return fail(h, MTZ_EINVAL, "COMPRESS: stream is already compressed");
+			if ((feat & FEAT_COMPRESSED) && !cin_on(h))
+				return fail(h, MTZ_EINVAL, "COMPRESS: stream is already compressed");
 			// the lz4-stage-v1 wire puts a preamble in front of every BEGIN: BEGIN opens its batch
 			if (bc.cnt > 0) return 0;
 			bc.emit_pre = true;
-			bc.pre_flags = (feat & FEAT_LZ4) ? WIRE_F_ORIG_LZ4 : 0u;
+			bc.pre_flags = wire_orig_lz4(feat);
 		} else if (h->cfg.mode == MTZ_MODE_DECOMPRESS) {
 			if (!ws->pre_seen)
 				return fail(h, MTZ_EINVAL, "DECOMPRESS: stream was not produced by the COMPRESS stage");
@@ -1598,13 +1643,17 @@ static int32_t harvest(mtz_handle *h, Slot &s)
 				std::lock_guard<std::mutex> g(h->stats_mu);
 				if (bad < h->stats.bad_record) h->stats.bad_record = bad;
 			}
-			return fail(h, MTZ_ECODEC, "LZ4 frame of record %llu does not decode to drr_logical_size",
+			return fail(h, MTZ_ECODEC, "record %llu: its frame does not decode to drr_logical_size, or no decoder "
+			    "takes its compression",
 			    (unsigned long long)bad);
 		}
 		std::lock_guard<std::mutex> g(h->stats_mu);
 		h->stats.lz4_decoded += c.n_dec;
 		h->stats.lz4_encoded += c.n_enc;
 		h->stats.lz4_certified += c.n_cert;
+		h->cstats.lz4_passed += c.n_pass;
+		h->cstats.lzjb_decoded += c.n_lzjb;
+		h->cstats.zle_decoded += c.n_zle;
 	}
 	int32_t rc = account_result(h, *s.h_res, s.first_rec, s.nrec, s.bytes, s.out_bytes,
 	    block_on(h) ? &bp : nullptr);

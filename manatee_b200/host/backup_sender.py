@@ -121,6 +121,11 @@ class BackupSender(object):
         for j in jobs:
             j["wire"] = "lz4-stage-v1" if compress else "raw"
 
+    def _send_compressed(self, backupJob):
+        """`zfs send -c` for this job: gpu.sendCompressed is set and _decide_wire chose the stage wire"""
+        return bool(self._gpu and self._gpu.get("mode") == "compress" and self._gpu.get("sendCompressed")
+                    and backupJob is not None and backupJob.get("wire") == "lz4-stage-v1")
+
     def _make_stage(self, backupJob=None):
         if not self._gpu or self._gpu.get("mode", "off") == "off":
             return None
@@ -137,14 +142,17 @@ class BackupSender(object):
                                 block_frames=bool(g.get("blockFrames")),
                                 block_lzjb=bool(g.get("blockLzjb")),
                                 block_logical=bool(g.get("blockLogical")),
-                                lz4_hc=bool(g.get("lz4Hc")))
+                                lz4_hc=bool(g.get("lz4Hc")),
+                                compressed_input=self._send_compressed(backupJob))
 
     def _stage_stats(self, stage):
         """job.gpu: the stage counters, plus `blocks` (block-checksum counters) with
-        gpu.blockChecksums set"""
+        gpu.blockChecksums set and `compressed_in` (mtz_get_compressed_in_stats) with gpu.sendCompressed"""
         st = stage.stats()
         if self._gpu.get("blockChecksums"):
             st["blocks"] = stage.block_stats()
+        if self._gpu.get("sendCompressed"):
+            st["compressed_in"] = stage.compressed_in_stats()
         return st
 
     def _send_group(self, jobs):
@@ -226,7 +234,11 @@ class BackupSender(object):
             if sock is None and peer_socks is None:
                 self._decide_wire([backupJob])
                 sock = socket.create_connection((backupJob["host"], int(backupJob["port"])))
-            zfsSend = subprocess.Popen([self._zfsPath, "send", "-v", "-P", snapshot],
+            # gpu.sendCompressed: a compressed-wire job takes the disk frames (`zfs send -c`), which the
+            # COMPRESS stage forwards (LZ4) or decodes and re-encodes (lzjb / zle); every other job
+            # spawns the reference's command
+            flags = ["-c"] if self._send_compressed(backupJob) else []
+            zfsSend = subprocess.Popen([self._zfsPath, "send"] + flags + ["-v", "-P", snapshot],
                                        stdout=subprocess.PIPE, stderr=subprocess.PIPE, env=self._env)
             backupJob["size"] = None
             backupJob["done"] = 0

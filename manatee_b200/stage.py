@@ -22,7 +22,7 @@ class GpuSnapshotStage(object):
     def __init__(self, mode="verify", device=0, ring_bytes=0, batch_bytes=0, n_slots=0,
                  out_ring_bytes=0, flags=0, devices=None, block_checksums=False, block_sha256=False,
                  block_sha512=False, block_frames=False, block_lzjb=False, block_logical=False,
-                 lz4_hc=False):
+                 lz4_hc=False, compressed_input=False):
         """``devices`` = CUDA ordinals of a device group: the GPUs of one box run as ONE stage,
         batch b of the stream on ``devices[b % len(devices)]`` (mtz_config.devices[]).
         ``block_checksums`` = MTZ_FLAG_BLOCK_CKSUM: every DRR_WRITE is also checked against the
@@ -48,7 +48,12 @@ class GpuSnapshotStage(object):
         accepts it and does not change.  Only valid with ``block_checksums``.
         ``lz4_hc`` = MTZ_FLAG_LZ4_HC: COMPRESS encodes with the stage's high-ratio LZ4 encoder (about
         10 % fewer payload bytes on the wire for pg-like pages, frames any DECOMPRESS stage decodes);
-        the other modes accept it and do not change."""
+        the other modes accept it and do not change.
+        ``compressed_input`` = MTZ_FLAG_COMPRESSED_IN: COMPRESS takes a `zfs send -c` stream, forwards its
+        LZ4 records as they are, decodes its lzjb / zle records on the GPU and encodes them like raw ones,
+        and fails with ECODEC on any other compression; the wire is the same lz4-stage-v1 a stock
+        DECOMPRESS stage turns into the plain stream (``compressed_in_stats()``).  The other modes
+        accept it and do not change."""
         if block_checksums:
             flags |= N.FLAG_BLOCK_CKSUM
         if block_sha256:
@@ -63,6 +68,8 @@ class GpuSnapshotStage(object):
             flags |= N.FLAG_BLOCK_LOGICAL
         if lz4_hc:
             flags |= N.FLAG_LZ4_HC
+        if compressed_input:
+            flags |= N.FLAG_COMPRESSED_IN
         self._L = N.lib()
         self._h = C.c_void_p()
         cfg = N.Config()
@@ -122,6 +129,14 @@ class GpuSnapshotStage(object):
         st = N.BlockStats()
         st.struct_size = C.sizeof(N.BlockStats)
         self._check(self._L.mtz_get_block_stats(self._h, C.byref(st)))
+        return st.as_dict()
+
+    def compressed_in_stats(self):
+        """MTZ_FLAG_COMPRESSED_IN counters (mtz_get_compressed_in_stats): lz4_passed, lzjb_decoded,
+        zle_decoded; all zero without ``compressed_input``."""
+        st = N.CompressedInStats()
+        st.struct_size = C.sizeof(N.CompressedInStats)
+        self._check(self._L.mtz_get_compressed_in_stats(self._h, C.byref(st)))
         return st.as_dict()
 
     def end_checksum(self):

@@ -47,6 +47,11 @@ PARAMS = {
                                                            (dict(sha256=True, sha512=True, lzjb=True),)],
     "test_a_corrupted_raw_keyed_lz4_record_fails_the_recompress_relay": [("fletcher4",), ("sha256",), ("sha512",)],
     "test_block_check_counts_the_hc_frames": [(False,), (True,)],
+    "test_output_equals_the_model": [("lz4-9", 8192), ("lz4-12", 8192), ("lzjb", 8192), ("zle", 8192),
+                                     ("mixed", 8192)],
+    "test_the_preamble_says_what_plain_send_would_have_said": [(0, False), (0, True), (1 << 16, False),
+                                                               (1 << 16, True)],
+    "test_block_counters_are_those_of_verify": [(False,), (True,)],
 }
 SKIP = {"test_sixteen_mib_record": "16 MiB blocks take minutes per encode on the emulator",
         "test_size_independent_properties_at_2gib": "2 GiB of LZ4 work is out of reach for the emulator",
@@ -79,12 +84,13 @@ def main():
     import test_gpu_block_lzjb as J
     import test_gpu_block_logical as L
     import test_gpu_codec as K
+    import test_gpu_compressed_in as CI
     import test_gpu_lz4 as Z
     import test_gpu_lz4hc as HC
     import test_gpu_stream as S
     import test_gpu_verify as V
     tot = fail = 0
-    for mod in (V, S, Z, K, B, H, W, F, J, L, HC):
+    for mod in (V, S, Z, K, B, H, W, F, J, L, HC, CI):
         for name, fn in inspect.getmembers(mod, inspect.isfunction):
             if not name.startswith("test_") or filt not in name:
                 continue

@@ -7,6 +7,8 @@ config 1): selected through the reference's own `zfsPath` knob
   zfs list -t snapshot -H -d 1 -S name -o name <ds>   -> <ds>@<13 digits> lines
   zfs send -v -P <snap>    -> stream from $FAKE_ZFS_STREAM on stdout, the
                               `full/size/HH:MM:SS` progress protocol on stderr
+  zfs send -c -v -P <snap> -> the same, from $FAKE_ZFS_STREAM_C when it is set
+                              ($FAKE_ZFS_SEND_ARGS: every send appends its arguments, one JSON list a line)
   zfs recv -v -u <ds>      -> drains stdin, writes sha256 + byte count to $FAKE_ZFS_RECV_OUT
 
 With $FAKE_ZFS_STATE (a JSON file, flock-protected) it also keeps a tiny pool model
@@ -216,8 +218,13 @@ def main():
         if stateful:
             with state() as st:
                 st["held"].append(snap)
+        if os.environ.get("FAKE_ZFS_SEND_ARGS"):
+            with open(os.environ["FAKE_ZFS_SEND_ARGS"], "a") as f:
+                f.write(json.dumps(a) + "\n")
         try:
             path = os.environ["FAKE_ZFS_STREAM"]
+            if "-c" in a[1:-1] and os.environ.get("FAKE_ZFS_STREAM_C"):
+                path = os.environ["FAKE_ZFS_STREAM_C"]
             size = os.path.getsize(path)
             sys.stderr.write("full\t%s\t%d\nsize\t%d\n" % (snap, size, size))
             sys.stderr.flush()

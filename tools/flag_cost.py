@@ -22,6 +22,11 @@ power limit and max SM clock the numbers were taken on.
                  DECOMPRESS of lzjb-keyed records (at --gib and at --large-gib), resident RECOMPRESS of
                  the compressed form of raw-keyed records (fletcher4 and sha256 keys), host COMPRESS
   lz4hc          MTZ_FLAG_LZ4_HC against COMPRESS without it: wire bytes, ratio and time, resident and host
+  compressed_in  MTZ_FLAG_COMPRESSED_IN: COMPRESS of the `zfs send -c` stream x with the flag against COMPRESS
+                 of plain(x), the stream today's sender pipes, for pg-page 128 KiB records written with lz4
+                 at ashift 9 and 12, lzjb, zle and block_ref.mixed_codecs: resident step, mtz_process_host
+                 and the ring API fed through a pipe (bench.py's ring_run, producer "pipe"), in GB/s of
+                 logical bytes; input and wire bytes, the counters, and the decoders' device time
 
 A resident step is timed with CUDA events around dev_submit + dev_finish on a side stream, a host pass
 with the host clock around mtz_process_host; kernel device times come from torch.profiler in a pass of
@@ -237,24 +242,27 @@ def synth(gib, kind, rs=RECSIZE):
     return O.synth_stream(max(1, int(gib * (1 << 30)) // (rs + 312)), rs, kind, nthreads=NTH)
 
 
-def keyed(O, s, threads, codec):
-    """block_ref.as_on_disk(O, s, 9, codec)[0] for codec DC_LZ4, DC_LZJB or DC_ZLE, with the frames and
-    their Fletcher-4 taken on `threads` threads (the C encoders and checksum release the GIL)"""
+def keyed(O, s, threads, codec, ashift=9):
+    """block_ref.as_on_disk(O, s, ashift, codec)[0] for codec DC_LZ4, DC_LZJB or DC_ZLE (or a function of
+    the record index that returns one), with the frames and their Fletcher-4 taken on `threads` threads
+    (the C encoders and checksum release the GIL)"""
     import numpy as np
     s = np.array(s, dtype=np.uint8, copy=True)
-    todo = [(off, po, pl) for off, po, pl, t in R.records(s) if t == 3 and s[off + 50] == 0]
+    pick = codec if callable(codec) else (lambda i: codec)
+    todo = [(i, off, po, pl) for i, (off, po, pl, t) in enumerate(R.records(s)) if t == 3 and s[off + 50] == 0]
 
     def key(job):
-        _, po, pl = job
+        i, _, po, pl = job
         logical = s[po:po + pl]
-        fr = R.disk_frame(O, logical, 9, codec)
+        dc = pick(i)
+        fr = None if dc == R.DC_OFF else R.disk_frame(O, logical, ashift, dc)
         if fr is None:
             return O.fletcher4(logical), R.prop(pl, pl, R.DC_OFF)
-        return O.fletcher4(np.ascontiguousarray(fr)), R.prop(pl, fr.size, codec)
+        return O.fletcher4(np.ascontiguousarray(fr)), R.prop(pl, fr.size, dc)
 
     with ThreadPoolExecutor(threads) as ex:
         keys = list(ex.map(key, todo, chunksize=256))
-    for (off, _, _), (k, p) in zip(todo, keys):
+    for (_, off, _, _), (k, p) in zip(todo, keys):
         R.set_key(s, off, R.FLETCHER4, k, p)
     assert O.stream_restamp(s)[0] == 0
     return s
@@ -369,6 +377,101 @@ def lz4hc(a):
     return res
 
 
+CIN_STREAMS = (("lz4_ashift9", R.DC_LZ4, 9), ("lz4_ashift12", R.DC_LZ4, 12), ("lzjb", R.DC_LZJB, 9),
+               ("zle", R.DC_ZLE, 9), ("mixed_codecs", R.mixed_codecs, 9))
+
+
+def compressed_in(a):
+    """each leg COMPRESSes its own form of the same data: "plain" the stream today's sender pipes (plain(x),
+    which for these streams is the keyed stream itself), "send_c" the `zfs send -c` stream x with the flag.
+    Both wires decode to the same plain stream; the check here is that the "send_c" wire DECOMPRESSes
+    to the "plain" leg's input."""
+    import numpy as np
+    import torch
+    import bench
+    from manatee_b200 import GpuSnapshotStage, index_host
+    names = ("plain", "send_c")
+    kw = {"plain": {}, "send_c": {"compressed_input": True}}
+    res = {"payload": "pg-page 128 KiB records (oracle.gen_payload(PAYLOAD_PGPAGE, r, 131072))"}
+    for sname, codec, ashift in CIN_STREAMS:
+        p = keyed(O, synth(a.gib, O.PAYLOAD_PGPAGE), NTH, codec, ashift)
+        x = R.as_send_c(O, p, ashift)
+        src = {"plain": p, "send_c": x}
+        logical = int(index_host(p)[0]["lsize"].sum())
+        r = {"logical_bytes": logical, "plain_bytes": int(p.size), "send_c_bytes": int(x.size)}
+        # resident steps, alternating
+        bufs = {}
+        for n in names:
+            recs, _ = index_host(src[n])
+            d_in = torch.from_numpy(src[n]).cuda()
+            d_recs = torch.from_numpy(recs.view(np.uint8).copy()).cuda()
+            cap = int(np.maximum(recs["lsize"], recs["payload"]).sum()) + 312 * len(recs) + (1 << 20)
+            bufs[n] = (d_in, d_recs, len(recs), torch.empty(cap, dtype=torch.uint8, device="cuda"), cap)
+        st = torch.cuda.Stream()
+        ms, wire = {n: [] for n in names}, {}
+        with ExitStack() as es:
+            gs = {n: es.enter_context(GpuSnapshotStage("compress", **kw[n])) for n in names}
+
+            def step(n):
+                g, (d_in, d_recs, nrec, d_out, cap) = gs[n], bufs[n]
+                g.dev_reset()
+                torch.cuda.synchronize()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(st)
+                g.dev_submit(d_in.data_ptr(), d_in.numel(), d_recs.data_ptr(), nrec, d_out.data_ptr(), cap,
+                             cuda_stream=st.cuda_stream)
+                ob = g.dev_finish()[0]
+                e1.record(st)
+                torch.cuda.synchronize()
+                return e0.elapsed_time(e1), ob
+
+            for i, n in alternate(kw, a.warmup + a.steps):
+                t, ob = step(n)
+                if i >= a.warmup:
+                    ms[n].append(t)
+                wire[n] = ob
+            r["resident"] = summary(names, ms, logical, "logical_gbps")
+            for n in names:
+                r["resident"][n + "_wire_bytes"] = int(wire[n])
+                r["resident"][n + "_lz4_encoded"] = gs[n].stats()["lz4_encoded"]
+            r["compressed_in_stats"] = gs["send_c"].compressed_in_stats()
+            if a.profile_steps:
+                r["resident"].update(kernel_times(partial(step, "send_c"), a.profile_steps,
+                                                  ("k_lzjb_decode", "k_zle_decode", "k3_lz4_encode")))
+        del bufs
+        torch.cuda.empty_cache()
+        # mtz_process_host, alternating; the send_c wire must decode to the plain stream
+        out = np.zeros(p.size + (64 << 20), dtype=np.uint8)
+        hms = {n: [] for n in names}
+        with ExitStack() as es:
+            gs = {n: es.enter_context(GpuSnapshotStage("compress", **kw[n])) for n in names}
+            for i, n in alternate(kw, 1 + a.host_steps):
+                t0 = time.perf_counter()
+                ob = gs[n].process_host(src[n], out)
+                if i >= 1:
+                    hms[n].append((time.perf_counter() - t0) * 1e3)
+                r[n + "_host_wire_bytes"] = int(ob)
+            with GpuSnapshotStage("decompress") as d:
+                back = np.zeros(p.size + (1 << 20), dtype=np.uint8)
+                nb = d.process_host(out[:ob], back)
+                r["decompressed_equals_plain"] = bool(nb == p.size and np.array_equal(back[:nb], p))
+        r["host"] = summary(names, hms, logical, "logical_gbps")
+        del out
+        # the ring API fed through a pipe: the shape of zfsSend.stdout
+        secs = {n: [] for n in names}
+        for _, n in alternate(kw, a.ring_steps):
+            with GpuSnapshotStage("compress", **kw[n]) as g:
+                dt, ok, detail = bench.ring_run(g, src[n], producer="pipe")
+                assert ok, detail
+                secs[n].append(dt)
+        r["ring_pipe"] = {n + "_logical_gbps_mean": logical / (sum(v) / len(v)) / 1e9 for n, v in secs.items()}
+        r["ring_pipe"].update({n + "_input_gbps_mean": src[n].size / (sum(v) / len(v)) / 1e9
+                               for n, v in secs.items()})
+        res[sname] = r
+        del p, x, src
+    return res
+
+
 SHA_OPTIONS = dict(verify_gib=16.0, host_gib=2.0, recompress_gib=1.0, steps=10, warmup=2, host_steps=4,
                    profile_steps=3)
 FRAME_OPTIONS = dict(verify_gib=16.0, host_gib=2.0, ring_gib=8.0, steps=10, warmup=2, host_steps=4, ring_steps=3,
@@ -383,6 +486,7 @@ WORKLOADS = {
     "block_logical": (block_logical, dict(gib=1.0, large_gib=4.0, host_gib=2.0, steps=10, warmup=2, host_steps=4,
                                           profile_steps=3)),
     "lz4hc": (lz4hc, dict(gib=1.0, host_gib=1.0, steps=5, warmup=1, host_steps=3, profile_steps=2)),
+    "compressed_in": (compressed_in, dict(gib=0.5, steps=5, warmup=1, host_steps=3, ring_steps=3, profile_steps=2)),
 }
 
 
