@@ -39,7 +39,8 @@ extern "C" {
 #define MTZ_EFORMAT  -4   /* malformed send stream (bad magic / type / length) */
 #define MTZ_ECKSUM   -5   /* embedded or END Fletcher-4 mismatch (like zfs recv ECKSUM) */
 #define MTZ_ECODEC   -6   /* LZ4 frame does not decode to drr_logical_size (MTZ_FLAG_COMPRESSED_IN: an
-                           * lzjb / zle frame, or a compression the stage has no decoder for) */
+                           * lzjb / zle frame, with MTZ_FLAG_GZIP_IN a gzip frame, or a compression
+                           * the stage has no decoder for) */
 #define MTZ_ENOSPC   -7   /* output capacity exceeded */
 #define MTZ_ENOMEM   -8
 #define MTZ_EOF      -9   /* consumer: stream finished and fully drained */
@@ -149,6 +150,21 @@ extern "C" {
                                   * mtz_get_compressed_in_stats.  VERIFY, DECOMPRESS, RECOMPRESS and
                                   * PASSTHROUGH accept the flag and do not change */
 
+#define MTZ_FLAG_GZIP_IN 1024u   /* with MTZ_FLAG_COMPRESSED_IN only (MTZ_EINVAL without it).  COMPRESS: a
+                                  * DRR_WRITE with drr_compressiontype 5..13 (gzip-1 .. gzip-9) is inflated
+                                  * on the GPU to drr_logical_size bytes, then stored LZ4 or raw like a raw
+                                  * record (K3, or K3h with MTZ_FLAG_LZ4_HC).  Acceptance is zlib's, strict on
+                                  * length: inflate of [payload, payload + drr_compressed_size) reaches the
+                                  * end of the stream, Adler-32 trailer included, inside the payload and
+                                  * gives exactly drr_logical_size bytes; the bytes after the trailer are
+                                  * ignored; anything else is MTZ_ECODEC at that record.  With
+                                  * MTZ_FLAG_BLOCK_CKSUM a record whose key says gzip-N on disk and that
+                                  * arrives as that frame is compared as it is (frame_ok or frame_miss,
+                                  * never an error); without this flag such keys are skipped.  Counters:
+                                  * mtz_compressed_in_stats.gzip_decoded.  Without this flag gzip records
+                                  * stay MTZ_ECODEC.  VERIFY, DECOMPRESS, RECOMPRESS and PASSTHROUGH accept
+                                  * the flag and do not change */
+
 typedef struct mtz_handle mtz_handle;
 
 #define MTZ_MAX_DEVICES 16
@@ -227,6 +243,8 @@ typedef struct mtz_compressed_in_stats {
 	uint64_t lz4_passed;        /* DRR_WRITEs that arrived LZ4 and were forwarded as they are */
 	uint64_t lzjb_decoded;      /* ... that arrived lzjb and were decoded on the GPU */
 	uint64_t zle_decoded;       /* ... that arrived zle and were decoded on the GPU */
+	uint64_t gzip_decoded;      /* MTZ_FLAG_GZIP_IN: ... that arrived gzip-1 .. gzip-9 and were inflated on
+	                               the GPU */
 } mtz_compressed_in_stats;
 
 /* One DRR record as seen by the kernels (32 B, little endian). */

@@ -32,6 +32,11 @@ namespace mtz {
                                // bytes they hold (k_logical_plan, kernels_frames.cuh)
 #define BLK_FR_CIN     8u      // COMPRESS with MTZ_FLAG_COMPRESSED_IN: with BLK_FR_LZJB, lzjb / zle records that
                                // arrive as their disk frame are compared as they are, as in VERIFY
+#define BLK_FR_GZIP    16u     // COMPRESS with MTZ_FLAG_COMPRESSED_IN | MTZ_FLAG_GZIP_IN: gzip-N records
+                               // (on-disk compression 5..13) that arrive as their disk frame are compared
+                               // as they are
+#define BLK_DC_GZIP1   5u
+#define BLK_DC_GZIP9   13u
 // BlockClass.src: where the bytes a key is compared with are
 #define BLK_SRC_IN     0       // the input payload
 #define BLK_SRC_OUT    1       // the output payload of a re-encoding mode
@@ -74,7 +79,8 @@ __host__ __device__ __forceinline__ Ck4 strip_head8(const Ck4 &whole, const Ck4 
 // BLK_FR_LZJB (MTZ_FLAG_BLOCK_LZJB) lzjb and zle keys are checked: against the input payload when
 // the record arrives as that frame (VERIFY, RECOMPRESS: passed through; COMPRESS with BLK_FR_CIN: before
 // it is decoded), in VERIFY against the
-// encoder's frame of a raw record.  With BLK_FR_LOGICAL the re-encoding modes also use the logical
+// encoder's frame of a raw record.  With BLK_FR_GZIP a gzip-N key of a record that arrives as that frame
+// is compared with the input payload.  With BLK_FR_LOGICAL the re-encoding modes also use the logical
 // bytes they hold (the raw input payload, or in DECOMPRESS and RECOMPRESS K2's output for a record that
 // arrives LZ4; COMPRESS decodes nothing, so an LZ4 record it is handed stays skipped), rows marked
 // `logical`: a raw-on-disk key of an LZ4 record in RECOMPRESS is compared with them; with BLK_FR_LZJB
@@ -118,6 +124,8 @@ __device__ __forceinline__ BlockClass block_classify(const uint8_t *hdr, const m
 			}
 			else if (raw_in && mode == MTZ_MODE_VERIFY) { c.what = 2; c.src = BLK_SRC_JOB; }
 			else if ((raw_in || lz4_in) && logical) { c.what = 2; c.src = BLK_SRC_JOB; c.logical = true; }
+		} else if ((frames & BLK_FR_GZIP) && dc >= BLK_DC_GZIP1 && dc <= BLK_DC_GZIP9) {
+			if (rec.comp == dc) { c.what = 2; c.src = BLK_SRC_IN; }
 		}
 	}
 	return c;

@@ -15,7 +15,8 @@
 namespace mtz {
 
 #define CF_DEC    1u      // payload is a frame that this mode decodes: ZFS-LZ4 (K2), or in COMPRESS with
-                          // MTZ_FLAG_COMPRESSED_IN lzjb / zle (k_lzjb_decode / k_zle_decode)
+                          // MTZ_FLAG_COMPRESSED_IN lzjb / zle (k_lzjb_decode / k_zle_decode) and with
+                          // MTZ_FLAG_GZIP_IN gzip-1 .. gzip-9 (k_inflate)
 #define CF_ENC    2u      // (decoded or raw) logical payload is offered to the encoder
 #define CF_WRITE  4u
 #define CF_PASS   8u      // COMPRESS with MTZ_FLAG_COMPRESSED_IN: an LZ4 frame forwarded as it is
@@ -52,17 +53,20 @@ struct CodecResult {       // device, mirrored to pinned host
 	uint32_t n_pass;       // COMPRESS with MTZ_FLAG_COMPRESSED_IN: LZ4 records forwarded as they are
 	uint32_t n_lzjb;       // ... lzjb records decoded (not counted in n_dec)
 	uint32_t n_zle;        // ... zle records decoded (likewise)
-	uint32_t pad;
+	uint32_t n_gzip;       // ... with MTZ_FLAG_GZIP_IN gzip records inflated (likewise)
 };
 
 // ---- plan, step 1: flags + scratch need -----------------------------------
-// `cin`: COMPRESS with MTZ_FLAG_COMPRESSED_IN.  The one place that decides what becomes of a
-// compressed DRR_WRITE there: lzjb / zle are decoded and offered to the encoder like a raw record,
-// LZ4 is forwarded as it is, any other compression fails the record (MTZ_ECODEC).
+// `cin`: COMPRESS with MTZ_FLAG_COMPRESSED_IN, `gzip`: ... and MTZ_FLAG_GZIP_IN.  The one place that
+// decides what becomes of a compressed DRR_WRITE there: lzjb / zle, and gzip-1 .. gzip-9 with `gzip`,
+// are decoded and offered to the encoder like a raw record, LZ4 is forwarded as it is, any other
+// compression fails the record (MTZ_ECODEC).
 #define ZIO_LZJB 3u
 #define ZIO_ZLE  14u
+#define ZIO_GZIP1 5u
+#define ZIO_GZIP9 13u
 __global__ void k_plan_need(const mtz_rec *__restrict__ recs, uint32_t n, uint32_t mode,
-    CodecRec *__restrict__ cr, uint64_t *__restrict__ vals, bool cin = false)
+    CodecRec *__restrict__ cr, uint64_t *__restrict__ vals, bool cin = false, bool gzip = false)
 {
 	const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
 	if (r >= n) return;
@@ -73,7 +77,9 @@ __global__ void k_plan_need(const mtz_rec *__restrict__ recs, uint32_t n, uint32
 		if (rec.comp == ZIO_LZ4 && (mode == MTZ_MODE_DECOMPRESS || mode == MTZ_MODE_RECOMPRESS))
 			f |= CF_DEC;
 		if (cin && mode == MTZ_MODE_COMPRESS && rec.comp != 0u)
-			f |= rec.comp == ZIO_LZJB || rec.comp == ZIO_ZLE ? CF_DEC : rec.comp == ZIO_LZ4 ? CF_PASS : CF_BAD;
+			f |= rec.comp == ZIO_LZJB || rec.comp == ZIO_ZLE ||
+			     (gzip && rec.comp >= ZIO_GZIP1 && rec.comp <= ZIO_GZIP9) ? CF_DEC :
+			     rec.comp == ZIO_LZ4 ? CF_PASS : CF_BAD;
 		if ((mode == MTZ_MODE_COMPRESS || mode == MTZ_MODE_RECOMPRESS) &&
 		    (rec.comp == 0u || (f & CF_DEC)))
 			f |= CF_ENC;
@@ -172,7 +178,8 @@ __global__ void k_layout(const mtz_rec *__restrict__ recs, uint32_t n, CodecRec 
 	if (c.flags & CF_BAD) atomicMin(&res->bad, r + rec_base);      // stays as it is: the batch fails
 	if (c.flags & CF_DEC) {
 		if (dec[r].status != MTZ_OK) atomicMin(&res->bad, r + rec_base);
-		else atomicAdd(rec.comp == ZIO_LZJB ? &res->n_lzjb : rec.comp == ZIO_ZLE ? &res->n_zle : &res->n_dec, 1u);
+		else atomicAdd(rec.comp == ZIO_LZJB ? &res->n_lzjb : rec.comp == ZIO_ZLE ? &res->n_zle :
+		    rec.comp >= ZIO_GZIP1 && rec.comp <= ZIO_GZIP9 ? &res->n_gzip : &res->n_dec, 1u);
 		len = rec.lsize;
 	}
 	if (c.flags & CF_PASS) atomicAdd(&res->n_pass, 1u);

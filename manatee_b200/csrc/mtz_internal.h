@@ -19,6 +19,7 @@
 #include "kernels_sha256.cuh"
 #include "kernels_sha512.cuh"
 #include "kernels_frames.cuh"
+#include "kernels_inflate.cuh"
 
 namespace mtz {
 

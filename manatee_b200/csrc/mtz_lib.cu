@@ -312,6 +312,8 @@ int32_t mtz_open(const mtz_config *cfg, mtz_handle **out)
 		return fail(nullptr, MTZ_EINVAL, "BLOCK_LZJB extends the block check: it needs BLOCK_CKSUM");
 	if ((full.flags & MTZ_FLAG_BLOCK_LOGICAL) && !(full.flags & MTZ_FLAG_BLOCK_CKSUM))
 		return fail(nullptr, MTZ_EINVAL, "BLOCK_LOGICAL extends the block check: it needs BLOCK_CKSUM");
+	if ((full.flags & MTZ_FLAG_GZIP_IN) && !(full.flags & MTZ_FLAG_COMPRESSED_IN))
+		return fail(nullptr, MTZ_EINVAL, "GZIP_IN extends COMPRESSED_IN: it needs COMPRESSED_IN");
 	const cudaDeviceProp &prop = props[0];
 
 	mtz_handle *h = new (std::nothrow) mtz_handle();
@@ -587,6 +589,7 @@ static bool block_frames_on(const mtz_handle *h)
 static bool block_lzjb_on(const mtz_handle *h) { return (h->cfg.flags & MTZ_FLAG_BLOCK_LZJB) != 0; }
 static bool is_codec_mode(uint32_t m);
 static bool cin_on(const mtz_handle *h);
+static bool gzip_on(const mtz_handle *h);
 // COMPRESS / DECOMPRESS / RECOMPRESS with MTZ_FLAG_BLOCK_LOGICAL: the block check runs jobs over the
 // logical bytes (launch_block_logical); VERIFY accepts the flag and does not change
 static bool block_logical_on(const mtz_handle *h)
@@ -600,7 +603,7 @@ static uint32_t block_fcodecs(const mtz_handle *h)
 {
 	return ((h->cfg.flags & MTZ_FLAG_BLOCK_FRAMES) && h->cfg.mode == MTZ_MODE_VERIFY ? BLK_FR_LZ4 : 0u) |
 	    (block_lzjb_on(h) ? BLK_FR_LZJB : 0u) | (block_logical_on(h) ? BLK_FR_LOGICAL : 0u) |
-	    (cin_on(h) ? BLK_FR_CIN : 0u);
+	    (cin_on(h) ? BLK_FR_CIN : 0u) | (gzip_on(h) ? BLK_FR_GZIP : 0u);
 }
 static uint32_t block_hashed(const mtz_handle *h)
 {
@@ -801,6 +804,12 @@ static bool cin_on(const mtz_handle *h)
 	return h->cfg.mode == MTZ_MODE_COMPRESS && (h->cfg.flags & MTZ_FLAG_COMPRESSED_IN) != 0;
 }
 
+// ... and with MTZ_FLAG_GZIP_IN its gzip-1 .. gzip-9 records are inflated (k_inflate) and re-encoded
+static bool gzip_on(const mtz_handle *h)
+{
+	return cin_on(h) && (h->cfg.flags & MTZ_FLAG_GZIP_IN) != 0;
+}
+
 // K3h's hash tables: one per warp of its persistent grid (launch_k3h)
 static size_t hc_tab_bytes(const mtz_handle *h)
 {
@@ -901,7 +910,8 @@ static int32_t codec_launch_pre(mtz_handle *h, cudaStream_t st, CodecBufs &cb, c
 }
 
 // plan + K2 (decode) of one (sub-)batch; in COMPRESS with MTZ_FLAG_COMPRESSED_IN the lzjb and zle
-// decoders in K2's place (every decode job of that mode is one of theirs)
+// decoders, and with MTZ_FLAG_GZIP_IN k_inflate, in K2's place (every decode job of that mode is one
+// of theirs)
 static int32_t codec_launch_dec(mtz_handle *h, cudaStream_t st, CodecBufs &cb, const uint8_t *d_in,
     const mtz_rec *d_recs, size_t nrec)
 {
@@ -909,7 +919,7 @@ static int32_t codec_launch_dec(mtz_handle *h, cudaStream_t st, CodecBufs &cb, c
 	if (nrec > cb.rec_cap) return fail(h, MTZ_ENOSPC, "codec batch of %zu records exceeds %zu", nrec, cb.rec_cap);
 	const uint32_t n = (uint32_t)nrec, mode = h->cfg.mode;
 	const unsigned tb = 256, gb = (n + tb - 1) / tb;
-	k_plan_need<<<gb, tb, 0, st>>>(d_recs, n, mode, cb.cr, cb.vals, cin_on(h));
+	k_plan_need<<<gb, tb, 0, st>>>(d_recs, n, mode, cb.cr, cb.vals, cin_on(h), gzip_on(h));
 	k_xscan_u64<<<1, XSCAN_THREADS, 0, st>>>(cb.vals, cb.offs, n, nullptr, nullptr);
 	k_plan_jobs<<<gb, tb, 0, st>>>(d_in, d_recs, n, cb.cr, cb.offs, cb.d_logical, cb.d_enc, cb.dec, cb.enc);
 	MTZ_CU(h, cudaGetLastError());
@@ -923,6 +933,12 @@ static int32_t codec_launch_dec(mtz_handle *h, cudaStream_t st, CodecBufs &cb, c
 		k_zle_decode<<<gl, LZJB_THREADS, 0, st>>>(d_recs, cb.dec, n);
 		MTZ_CU(h, cudaGetLastError());
 		count_launch(h, 2);
+		if (gzip_on(h)) {
+			const unsigned gi = (unsigned)std::min<size_t>((nrec + INFL_WARPS - 1) / INFL_WARPS, (size_t)h->sm_count * 8);
+			k_inflate<<<gi, INFL_THREADS, 0, st>>>(d_recs, cb.dec, n);
+			MTZ_CU(h, cudaGetLastError());
+			count_launch(h, 1);
+		}
 	}
 	return MTZ_OK;
 }
@@ -1478,6 +1494,7 @@ static int32_t dev_finish_impl(mtz_handle *h, const uint64_t carry_in[4], const 
 		h->cstats.lz4_passed += c.n_pass;
 		h->cstats.lzjb_decoded += c.n_lzjb;
 		h->cstats.zle_decoded += c.n_zle;
+		h->cstats.gzip_decoded += c.n_gzip;
 	}
 	if (out_bytes) *out_bytes = ob;
 	rc = account_result(h, r, h->dv_first, h->dv_nrec, h->dv_in_bytes, ob, block_on(h) ? &h->bpend : nullptr);
@@ -1654,6 +1671,7 @@ static int32_t harvest(mtz_handle *h, Slot &s)
 		h->cstats.lz4_passed += c.n_pass;
 		h->cstats.lzjb_decoded += c.n_lzjb;
 		h->cstats.zle_decoded += c.n_zle;
+		h->cstats.gzip_decoded += c.n_gzip;
 	}
 	int32_t rc = account_result(h, *s.h_res, s.first_rec, s.nrec, s.bytes, s.out_bytes,
 	    block_on(h) ? &bp : nullptr);

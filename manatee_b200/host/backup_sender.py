@@ -143,11 +143,13 @@ class BackupSender(object):
                                 block_lzjb=bool(g.get("blockLzjb")),
                                 block_logical=bool(g.get("blockLogical")),
                                 lz4_hc=bool(g.get("lz4Hc")),
-                                compressed_input=self._send_compressed(backupJob))
+                                compressed_input=self._send_compressed(backupJob),
+                                gzip_input=self._send_compressed(backupJob) and bool(g.get("sendGzip")))
 
     def _stage_stats(self, stage):
         """job.gpu: the stage counters, plus `blocks` (block-checksum counters) with
-        gpu.blockChecksums set and `compressed_in` (mtz_get_compressed_in_stats) with gpu.sendCompressed"""
+        gpu.blockChecksums set and `compressed_in` (mtz_get_compressed_in_stats) with gpu.sendCompressed,
+        gzip_decoded included with gpu.sendGzip"""
         st = stage.stats()
         if self._gpu.get("blockChecksums"):
             st["blocks"] = stage.block_stats()
@@ -235,7 +237,8 @@ class BackupSender(object):
                 self._decide_wire([backupJob])
                 sock = socket.create_connection((backupJob["host"], int(backupJob["port"])))
             # gpu.sendCompressed: a compressed-wire job takes the disk frames (`zfs send -c`), which the
-            # COMPRESS stage forwards (LZ4) or decodes and re-encodes (lzjb / zle); every other job
+            # COMPRESS stage forwards (LZ4) or decodes and re-encodes (lzjb / zle, and gzip with
+            # gpu.sendGzip); every other job
             # spawns the reference's command
             flags = ["-c"] if self._send_compressed(backupJob) else []
             zfsSend = subprocess.Popen([self._zfsPath, "send"] + flags + ["-v", "-P", snapshot],

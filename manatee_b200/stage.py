@@ -22,7 +22,7 @@ class GpuSnapshotStage(object):
     def __init__(self, mode="verify", device=0, ring_bytes=0, batch_bytes=0, n_slots=0,
                  out_ring_bytes=0, flags=0, devices=None, block_checksums=False, block_sha256=False,
                  block_sha512=False, block_frames=False, block_lzjb=False, block_logical=False,
-                 lz4_hc=False, compressed_input=False):
+                 lz4_hc=False, compressed_input=False, gzip_input=False):
         """``devices`` = CUDA ordinals of a device group: the GPUs of one box run as ONE stage,
         batch b of the stream on ``devices[b % len(devices)]`` (mtz_config.devices[]).
         ``block_checksums`` = MTZ_FLAG_BLOCK_CKSUM: every DRR_WRITE is also checked against the
@@ -53,7 +53,11 @@ class GpuSnapshotStage(object):
         LZ4 records as they are, decodes its lzjb / zle records on the GPU and encodes them like raw ones,
         and fails with ECODEC on any other compression; the wire is the same lz4-stage-v1 a stock
         DECOMPRESS stage turns into the plain stream (``compressed_in_stats()``).  The other modes
-        accept it and do not change."""
+        accept it and do not change.
+        ``gzip_input`` = MTZ_FLAG_GZIP_IN, only valid with ``compressed_input``: COMPRESS also inflates
+        the gzip-1 .. gzip-9 records on the GPU and encodes them like raw ones; a frame zlib would not
+        inflate to exactly drr_logical_size bytes is ECODEC.  ``compressed_in_stats()`` then also
+        reports ``gzip_decoded``.  The other modes accept it and do not change."""
         if block_checksums:
             flags |= N.FLAG_BLOCK_CKSUM
         if block_sha256:
@@ -70,6 +74,9 @@ class GpuSnapshotStage(object):
             flags |= N.FLAG_LZ4_HC
         if compressed_input:
             flags |= N.FLAG_COMPRESSED_IN
+        if gzip_input:
+            flags |= N.FLAG_GZIP_IN
+        self._gzip_input = bool(gzip_input)
         self._L = N.lib()
         self._h = C.c_void_p()
         cfg = N.Config()
@@ -133,11 +140,15 @@ class GpuSnapshotStage(object):
 
     def compressed_in_stats(self):
         """MTZ_FLAG_COMPRESSED_IN counters (mtz_get_compressed_in_stats): lz4_passed, lzjb_decoded,
-        zle_decoded; all zero without ``compressed_input``."""
+        zle_decoded, and gzip_decoded for a stage opened with ``gzip_input``; all zero without
+        ``compressed_input``."""
         st = N.CompressedInStats()
         st.struct_size = C.sizeof(N.CompressedInStats)
         self._check(self._L.mtz_get_compressed_in_stats(self._h, C.byref(st)))
-        return st.as_dict()
+        d = st.as_dict()
+        if not self._gzip_input:
+            del d["gzip_decoded"]
+        return d
 
     def end_checksum(self):
         out = (C.c_uint64 * 4)()

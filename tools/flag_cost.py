@@ -27,6 +27,9 @@ power limit and max SM clock the numbers were taken on.
                  at ashift 9 and 12, lzjb, zle and block_ref.mixed_codecs: resident step, mtz_process_host
                  and the ring API fed through a pipe (bench.py's ring_run, producer "pipe"), in GB/s of
                  logical bytes; input and wire bytes, the counters, and the decoders' device time
+  gzip_in        MTZ_FLAG_GZIP_IN: the same legs, the flag leg with compressed_input + gzip_input, for
+                 pg-page 128 KiB records written with gzip-1, gzip-6, gzip-9 and a gzip-6 / lz4 / lzjb /
+                 raw pool; plus k_inflate's device time and single-thread zlib.decompress of the records
 
 A resident step is timed with CUDA events around dev_submit + dev_finish on a side stream, a host pass
 with the host clock around mtz_process_host; kernel device times come from torch.profiler in a pass of
@@ -48,6 +51,8 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import block_ref as R  # noqa: E402
+import compressed_in_ref as CI  # noqa: E402
+import gzip_in_ref as GZ  # noqa: E402
 import oracle as O  # noqa: E402
 
 RECSIZE = 131072
@@ -243,9 +248,9 @@ def synth(gib, kind, rs=RECSIZE):
 
 
 def keyed(O, s, threads, codec, ashift=9):
-    """block_ref.as_on_disk(O, s, ashift, codec)[0] for codec DC_LZ4, DC_LZJB or DC_ZLE (or a function of
-    the record index that returns one), with the frames and their Fletcher-4 taken on `threads` threads
-    (the C encoders and checksum release the GIL)"""
+    """block_ref.as_on_disk(O, s, ashift, codec)[0] for codec DC_LZ4, DC_LZJB, DC_ZLE or gzip-N (or a
+    function of the record index that returns one), with the frames and their Fletcher-4 taken on
+    `threads` threads (the C encoders, zlib and checksum release the GIL)"""
     import numpy as np
     s = np.array(s, dtype=np.uint8, copy=True)
     pick = codec if callable(codec) else (lambda i: codec)
@@ -255,7 +260,7 @@ def keyed(O, s, threads, codec, ashift=9):
         i, _, po, pl = job
         logical = s[po:po + pl]
         dc = pick(i)
-        fr = None if dc == R.DC_OFF else R.disk_frame(O, logical, ashift, dc)
+        fr = None if dc == R.DC_OFF else GZ.disk_frame(O, logical, ashift, dc)
         if fr is None:
             return O.fletcher4(logical), R.prop(pl, pl, R.DC_OFF)
         return O.fletcher4(np.ascontiguousarray(fr)), R.prop(pl, fr.size, dc)
@@ -386,16 +391,22 @@ def compressed_in(a):
     which for these streams is the keyed stream itself), "send_c" the `zfs send -c` stream x with the flag.
     Both wires decode to the same plain stream; the check here is that the "send_c" wire DECOMPRESSes
     to the "plain" leg's input."""
+    return send_c_legs(a, CIN_STREAMS, {"compressed_input": True}, ("k_lzjb_decode", "k_zle_decode", "k3_lz4_encode"))
+
+
+def send_c_legs(a, streams, flag_kw, kernels, fields=None):
+    """compressed_in's legs over each of `streams` (name, codec, ashift), the "send_c" leg opened with
+    `flag_kw`; `fields(r, p, x)` adds a stream's own fields"""
     import numpy as np
     import torch
     import bench
     from manatee_b200 import GpuSnapshotStage, index_host
     names = ("plain", "send_c")
-    kw = {"plain": {}, "send_c": {"compressed_input": True}}
+    kw = {"plain": {}, "send_c": flag_kw}
     res = {"payload": "pg-page 128 KiB records (oracle.gen_payload(PAYLOAD_PGPAGE, r, 131072))"}
-    for sname, codec, ashift in CIN_STREAMS:
+    for sname, codec, ashift in streams:
         p = keyed(O, synth(a.gib, O.PAYLOAD_PGPAGE), NTH, codec, ashift)
-        x = R.as_send_c(O, p, ashift)
+        x = GZ.as_send_c(O, p, ashift)
         src = {"plain": p, "send_c": x}
         logical = int(index_host(p)[0]["lsize"].sum())
         r = {"logical_bytes": logical, "plain_bytes": int(p.size), "send_c_bytes": int(x.size)}
@@ -436,8 +447,7 @@ def compressed_in(a):
                 r["resident"][n + "_lz4_encoded"] = gs[n].stats()["lz4_encoded"]
             r["compressed_in_stats"] = gs["send_c"].compressed_in_stats()
             if a.profile_steps:
-                r["resident"].update(kernel_times(partial(step, "send_c"), a.profile_steps,
-                                                  ("k_lzjb_decode", "k_zle_decode", "k3_lz4_encode")))
+                r["resident"].update(kernel_times(partial(step, "send_c"), a.profile_steps, kernels))
         del bufs
         torch.cuda.empty_cache()
         # mtz_process_host, alternating; the send_c wire must decode to the plain stream
@@ -467,9 +477,34 @@ def compressed_in(a):
         r["ring_pipe"] = {n + "_logical_gbps_mean": logical / (sum(v) / len(v)) / 1e9 for n, v in secs.items()}
         r["ring_pipe"].update({n + "_input_gbps_mean": src[n].size / (sum(v) / len(v)) / 1e9
                                for n, v in secs.items()})
+        if fields is not None:
+            fields(r, p, x)
         res[sname] = r
         del p, x, src
     return res
+
+
+GZIP_STREAMS = (("gzip1", GZ.DC_GZIP[1], 9), ("gzip6", GZ.DC_GZIP[6], 9), ("gzip9", GZ.DC_GZIP[9], 9),
+                ("mixed_gzip6_lz4_lzjb_raw", lambda i: (GZ.DC_GZIP[6], R.DC_LZ4, R.DC_LZJB, R.DC_OFF)[i % 4], 9))
+
+
+def gzip_in(a):
+    """compressed_in's legs over gzip pools, the "send_c" leg with compressed_input + gzip_input; plus
+    the single-thread zlib.decompress rate of the same gzip records, as context for what the sending
+    host's CPU spends on them without -c"""
+    import zlib
+
+    def zlib_rate(r, p, x):
+        frames = [x[po:po + pl].tobytes() for _, off, po, pl in CI.write_records(x) if GZ.is_gzip(int(x[off + 50]))]
+        if not frames:
+            return
+        t0 = time.perf_counter()
+        n = sum(len(zlib.decompress(f)) for f in frames)
+        r["zlib_decompress_1thread_logical_gbps"] = n / (time.perf_counter() - t0) / 1e9
+        r["gzip_records"] = len(frames)
+
+    return send_c_legs(a, GZIP_STREAMS, {"compressed_input": True, "gzip_input": True},
+                       ("k_inflate", "k_lzjb_decode", "k3_lz4_encode"), zlib_rate)
 
 
 SHA_OPTIONS = dict(verify_gib=16.0, host_gib=2.0, recompress_gib=1.0, steps=10, warmup=2, host_steps=4,
@@ -487,6 +522,7 @@ WORKLOADS = {
                                           profile_steps=3)),
     "lz4hc": (lz4hc, dict(gib=1.0, host_gib=1.0, steps=5, warmup=1, host_steps=3, profile_steps=2)),
     "compressed_in": (compressed_in, dict(gib=0.5, steps=5, warmup=1, host_steps=3, ring_steps=3, profile_steps=2)),
+    "gzip_in": (gzip_in, dict(gib=0.5, steps=5, warmup=1, host_steps=3, ring_steps=3, profile_steps=2)),
 }
 
 
