@@ -40,7 +40,8 @@ extern "C" {
 #define MTZ_ECKSUM   -5   /* embedded or END Fletcher-4 mismatch (like zfs recv ECKSUM) */
 #define MTZ_ECODEC   -6   /* LZ4 frame does not decode to drr_logical_size (MTZ_FLAG_COMPRESSED_IN: an
                            * lzjb / zle frame, with MTZ_FLAG_GZIP_IN a gzip frame, or a compression
-                           * the stage has no decoder for) */
+                           * the stage has no decoder for; in DECOMPRESS with MTZ_FLAG_GZIP_WIRE a
+                           * gzip frame) */
 #define MTZ_ENOSPC   -7   /* output capacity exceeded */
 #define MTZ_ENOMEM   -8
 #define MTZ_EOF      -9   /* consumer: stream finished and fully drained */
@@ -165,6 +166,22 @@ extern "C" {
                                   * stay MTZ_ECODEC.  VERIFY, DECOMPRESS, RECOMPRESS and PASSTHROUGH accept
                                   * the flag and do not change */
 
+#define MTZ_FLAG_GZIP_WIRE 2048u /* gzip frames on the compressed wire.  Never with MTZ_FLAG_GZIP_IN
+                                  * (MTZ_EINVAL).  COMPRESS, with MTZ_FLAG_COMPRESSED_IN only (MTZ_EINVAL
+                                  * without it): a DRR_WRITE with drr_compressiontype 5..13 (gzip-1 ..
+                                  * gzip-9) is forwarded byte for byte like an LZ4 one, with only the stream
+                                  * checksum re-stamped (also under MTZ_FLAG_LZ4_HC), and every wire preamble
+                                  * carries the capability bit WIRE_F_GZIP (2).  DECOMPRESS: the preamble
+                                  * may carry that bit (without this flag it is MTZ_EFORMAT), and a gzip-1 ..
+                                  * gzip-9 DRR_WRITE is inflated on the GPU by MTZ_FLAG_GZIP_IN's rule
+                                  * (anything else is MTZ_ECODEC at that record) and leaves raw, as `zfs
+                                  * send` without -c would have written it; on every path, the device API
+                                  * included, since the flag is the handle's and not the preamble's.  With
+                                  * MTZ_FLAG_BLOCK_CKSUM both sides compare a gzip-N key of a record that
+                                  * arrives as that frame as it is.  Counters: mtz_compressed_in_stats
+                                  * .gzip_passed (COMPRESS) and .gzip_decoded (DECOMPRESS).  VERIFY,
+                                  * RECOMPRESS and PASSTHROUGH accept the flag and do not change */
+
 typedef struct mtz_handle mtz_handle;
 
 #define MTZ_MAX_DEVICES 16
@@ -244,7 +261,9 @@ typedef struct mtz_compressed_in_stats {
 	uint64_t lzjb_decoded;      /* ... that arrived lzjb and were decoded on the GPU */
 	uint64_t zle_decoded;       /* ... that arrived zle and were decoded on the GPU */
 	uint64_t gzip_decoded;      /* MTZ_FLAG_GZIP_IN: ... that arrived gzip-1 .. gzip-9 and were inflated on
-	                               the GPU */
+	                               the GPU; likewise in DECOMPRESS with MTZ_FLAG_GZIP_WIRE */
+	uint64_t gzip_passed;       /* COMPRESS with MTZ_FLAG_GZIP_WIRE: ... that arrived gzip-1 .. gzip-9 and
+	                               were forwarded as they are */
 } mtz_compressed_in_stats;
 
 /* One DRR record as seen by the kernels (32 B, little endian). */

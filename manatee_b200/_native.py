@@ -26,6 +26,7 @@ FLAG_BLOCK_LOGICAL = 128
 FLAG_LZ4_HC = 256
 FLAG_COMPRESSED_IN = 512
 FLAG_GZIP_IN = 1024
+FLAG_GZIP_WIRE = 2048
 XCHG_FIRST, XCHG_LAST = 1, 2
 MODE_NAMES = {"verify": 0, "compress": 1, "decompress": 2, "recompress": 3, "passthrough": 4}
 
@@ -70,7 +71,8 @@ class BlockStats(C.Structure):
 
 class CompressedInStats(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("pad", C.c_uint32), ("lz4_passed", C.c_uint64),
-                ("lzjb_decoded", C.c_uint64), ("zle_decoded", C.c_uint64), ("gzip_decoded", C.c_uint64)]
+                ("lzjb_decoded", C.c_uint64), ("zle_decoded", C.c_uint64), ("gzip_decoded", C.c_uint64),
+                ("gzip_passed", C.c_uint64)]
 
     def as_dict(self):
         return {k: getattr(self, k) for k, _ in self._fields_[2:]}

@@ -32,9 +32,10 @@ namespace mtz {
                                // bytes they hold (k_logical_plan, kernels_frames.cuh)
 #define BLK_FR_CIN     8u      // COMPRESS with MTZ_FLAG_COMPRESSED_IN: with BLK_FR_LZJB, lzjb / zle records that
                                // arrive as their disk frame are compared as they are, as in VERIFY
-#define BLK_FR_GZIP    16u     // COMPRESS with MTZ_FLAG_COMPRESSED_IN | MTZ_FLAG_GZIP_IN: gzip-N records
-                               // (on-disk compression 5..13) that arrive as their disk frame are compared
-                               // as they are
+#define BLK_FR_GZIP    16u     // COMPRESS with MTZ_FLAG_COMPRESSED_IN | MTZ_FLAG_GZIP_IN, or with
+                               // MTZ_FLAG_COMPRESSED_IN | MTZ_FLAG_GZIP_WIRE, and DECOMPRESS with
+                               // MTZ_FLAG_GZIP_WIRE: gzip-N records (on-disk compression 5..13) that arrive
+                               // as their disk frame are compared as they are
 #define BLK_DC_GZIP1   5u
 #define BLK_DC_GZIP9   13u
 // BlockClass.src: where the bytes a key is compared with are

@@ -16,10 +16,12 @@ namespace mtz {
 
 #define CF_DEC    1u      // payload is a frame that this mode decodes: ZFS-LZ4 (K2), or in COMPRESS with
                           // MTZ_FLAG_COMPRESSED_IN lzjb / zle (k_lzjb_decode / k_zle_decode) and with
-                          // MTZ_FLAG_GZIP_IN gzip-1 .. gzip-9 (k_inflate)
+                          // MTZ_FLAG_GZIP_IN gzip-1 .. gzip-9 (k_inflate); in DECOMPRESS with
+                          // MTZ_FLAG_GZIP_WIRE also gzip-1 .. gzip-9 (k_inflate over the second job table)
 #define CF_ENC    2u      // (decoded or raw) logical payload is offered to the encoder
 #define CF_WRITE  4u
-#define CF_PASS   8u      // COMPRESS with MTZ_FLAG_COMPRESSED_IN: an LZ4 frame forwarded as it is
+#define CF_PASS   8u      // COMPRESS with MTZ_FLAG_COMPRESSED_IN: an LZ4 frame, and with MTZ_FLAG_GZIP_WIRE
+                          // a gzip frame, forwarded as it is
 #define CF_BAD    16u     // ... a compression the stage cannot decode: its decode job fails
 
 #define FEAT_LZ4        (1ull << 17)
@@ -33,6 +35,8 @@ namespace mtz {
 #define WIRE_VERSION    1u
 #define WIRE_PRE_BYTES  32u
 #define WIRE_F_ORIG_LZ4 1u
+#define WIRE_F_GZIP     2u      // COMPRESS with MTZ_FLAG_GZIP_WIRE: gzip frames may follow.  Only a DECOMPRESS
+                                // opened with that flag accepts the bit; any other refuses the preamble
 #define ZIO_LZ4         15u
 
 struct CodecRec {          // 32 B per record, device only
@@ -53,20 +57,27 @@ struct CodecResult {       // device, mirrored to pinned host
 	uint32_t n_pass;       // COMPRESS with MTZ_FLAG_COMPRESSED_IN: LZ4 records forwarded as they are
 	uint32_t n_lzjb;       // ... lzjb records decoded (not counted in n_dec)
 	uint32_t n_zle;        // ... zle records decoded (likewise)
-	uint32_t n_gzip;       // ... with MTZ_FLAG_GZIP_IN gzip records inflated (likewise)
+	uint32_t n_gzip;       // ... with MTZ_FLAG_GZIP_IN gzip records inflated (likewise); also DECOMPRESS
+	                       // with MTZ_FLAG_GZIP_WIRE
+	uint32_t n_gzpass;     // COMPRESS with MTZ_FLAG_GZIP_WIRE: gzip records forwarded (not in n_pass)
+	uint32_t pad;
 };
 
 // ---- plan, step 1: flags + scratch need -----------------------------------
-// `cin`: COMPRESS with MTZ_FLAG_COMPRESSED_IN, `gzip`: ... and MTZ_FLAG_GZIP_IN.  The one place that
-// decides what becomes of a compressed DRR_WRITE there: lzjb / zle, and gzip-1 .. gzip-9 with `gzip`,
-// are decoded and offered to the encoder like a raw record, LZ4 is forwarded as it is, any other
-// compression fails the record (MTZ_ECODEC).
+// `cin`: COMPRESS with MTZ_FLAG_COMPRESSED_IN, `gzip`: ... and MTZ_FLAG_GZIP_IN, `gzwire`: the handle has
+// MTZ_FLAG_GZIP_WIRE.  The one place that decides what becomes of a compressed DRR_WRITE: in COMPRESS
+// with `cin` lzjb / zle, and gzip-1 .. gzip-9 with `gzip`, are decoded and offered to the encoder like
+// a raw record, LZ4, and gzip-1 .. gzip-9 with `gzwire`, are forwarded as they are, any other
+// compression fails the record (MTZ_ECODEC); in DECOMPRESS with `gzwire` gzip-1 .. gzip-9 are decoded
+// (k_inflate) and leave raw.
 #define ZIO_LZJB 3u
 #define ZIO_ZLE  14u
 #define ZIO_GZIP1 5u
 #define ZIO_GZIP9 13u
+__device__ __forceinline__ bool is_gzip(uint32_t comp) { return comp >= ZIO_GZIP1 && comp <= ZIO_GZIP9; }
 __global__ void k_plan_need(const mtz_rec *__restrict__ recs, uint32_t n, uint32_t mode,
-    CodecRec *__restrict__ cr, uint64_t *__restrict__ vals, bool cin = false, bool gzip = false)
+    CodecRec *__restrict__ cr, uint64_t *__restrict__ vals, bool cin = false, bool gzip = false,
+    bool gzwire = false)
 {
 	const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
 	if (r >= n) return;
@@ -74,12 +85,13 @@ __global__ void k_plan_need(const mtz_rec *__restrict__ recs, uint32_t n, uint32
 	uint32_t f = 0;
 	if (rec.type == DRR_WRITE_T) {
 		f |= CF_WRITE;
-		if (rec.comp == ZIO_LZ4 && (mode == MTZ_MODE_DECOMPRESS || mode == MTZ_MODE_RECOMPRESS))
+		const bool gz = is_gzip(rec.comp);
+		if ((rec.comp == ZIO_LZ4 && (mode == MTZ_MODE_DECOMPRESS || mode == MTZ_MODE_RECOMPRESS)) ||
+		    (gzwire && gz && mode == MTZ_MODE_DECOMPRESS))
 			f |= CF_DEC;
 		if (cin && mode == MTZ_MODE_COMPRESS && rec.comp != 0u)
-			f |= rec.comp == ZIO_LZJB || rec.comp == ZIO_ZLE ||
-			     (gzip && rec.comp >= ZIO_GZIP1 && rec.comp <= ZIO_GZIP9) ? CF_DEC :
-			     rec.comp == ZIO_LZ4 ? CF_PASS : CF_BAD;
+			f |= rec.comp == ZIO_LZJB || rec.comp == ZIO_ZLE || (gzip && gz) ? CF_DEC :
+			     rec.comp == ZIO_LZ4 || (gzwire && gz) ? CF_PASS : CF_BAD;
 		if ((mode == MTZ_MODE_COMPRESS || mode == MTZ_MODE_RECOMPRESS) &&
 		    (rec.comp == 0u || (f & CF_DEC)))
 			f |= CF_ENC;
@@ -134,9 +146,13 @@ k_xscan_u64(const uint64_t *__restrict__ in, uint64_t *__restrict__ out, uint32_
 }
 
 // ---- plan, step 2: jobs with absolute device addresses --------------------
+// With `dec_gz` (DECOMPRESS with MTZ_FLAG_GZIP_WIRE) the decode job of a gzip record goes there and its
+// slot of `dec` stays empty, so that K2, which decodes every job of `dec` with lsize != 0, never sees
+// it; k_inflate runs over `dec_gz`, whose other slots are empty.
 __global__ void k_plan_jobs(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs,
     uint32_t n, CodecRec *__restrict__ cr, const uint64_t *__restrict__ offs,
-    uint8_t *d_logical, uint8_t *d_enc, mtz_job *__restrict__ dec, mtz_job *__restrict__ enc)
+    uint8_t *d_logical, uint8_t *d_enc, mtz_job *__restrict__ dec, mtz_job *__restrict__ enc,
+    mtz_job *__restrict__ dec_gz = nullptr)
 {
 	const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
 	if (r >= n) return;
@@ -161,6 +177,13 @@ __global__ void k_plan_jobs(const uint8_t *__restrict__ d_in, const mtz_rec *__r
 		je.dst_off = (uint64_t)(uintptr_t)(d_enc + c.scratch);
 		je.lsize = rec.lsize;
 	}
+	if (dec_gz != nullptr) {
+		mtz_job none;
+		none.src_off = none.dst_off = 0; none.src_len = 0; none.lsize = 0; none.out_len = 0; none.status = 0;
+		const bool gz = is_gzip(rec.comp);
+		dec_gz[r] = gz ? jd : none;
+		if (gz) jd = none;
+	}
 	dec[r] = jd; enc[r] = je;
 }
 
@@ -168,7 +191,7 @@ __global__ void k_plan_jobs(const uint8_t *__restrict__ d_in, const mtz_rec *__r
 __global__ void k_layout(const mtz_rec *__restrict__ recs, uint32_t n, CodecRec *__restrict__ cr,
     const mtz_job *__restrict__ dec, const mtz_job *__restrict__ enc,
     uint64_t *__restrict__ vals, CodecResult *__restrict__ res, uint32_t rec_base,
-    const uint32_t *__restrict__ cert = nullptr)
+    const uint32_t *__restrict__ cert = nullptr, const mtz_job *__restrict__ dec_gz = nullptr)
 {
 	const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
 	if (r >= n) return;
@@ -176,13 +199,14 @@ __global__ void k_layout(const mtz_rec *__restrict__ recs, uint32_t n, CodecRec 
 	CodecRec c = cr[r];
 	uint32_t len = rec.payload;
 	if (c.flags & CF_BAD) atomicMin(&res->bad, r + rec_base);      // stays as it is: the batch fails
+	const bool gz = is_gzip(rec.comp);
 	if (c.flags & CF_DEC) {
-		if (dec[r].status != MTZ_OK) atomicMin(&res->bad, r + rec_base);
+		if ((dec_gz != nullptr && gz ? dec_gz[r] : dec[r]).status != MTZ_OK) atomicMin(&res->bad, r + rec_base);
 		else atomicAdd(rec.comp == ZIO_LZJB ? &res->n_lzjb : rec.comp == ZIO_ZLE ? &res->n_zle :
-		    rec.comp >= ZIO_GZIP1 && rec.comp <= ZIO_GZIP9 ? &res->n_gzip : &res->n_dec, 1u);
+		    gz ? &res->n_gzip : &res->n_dec, 1u);
 		len = rec.lsize;
 	}
-	if (c.flags & CF_PASS) atomicAdd(&res->n_pass, 1u);
+	if (c.flags & CF_PASS) atomicAdd(gz ? &res->n_gzpass : &res->n_pass, 1u);
 	if ((c.flags & CF_ENC) && enc[r].out_len < rec.lsize) {
 		len = enc[r].out_len;
 		atomicAdd(&res->n_enc, 1u);

@@ -37,8 +37,6 @@ struct InflSmem {
 	uint8_t lens[320];                // code lengths: literal/length then distance
 };
 
-__device__ __forceinline__ bool is_gzip(uint32_t comp) { return comp >= ZIO_GZIP1 && comp <= ZIO_GZIP9; }
-
 __device__ __forceinline__ uint32_t rev16(uint32_t v)
 {
 	v = ((v & 0x5555u) << 1) | ((v >> 1) & 0x5555u);

@@ -54,6 +54,7 @@ struct CodecBufs {
 	CodecRec *cr = nullptr;
 	uint64_t *vals = nullptr, *offs = nullptr, *out_offs = nullptr;
 	mtz_job *dec = nullptr, *enc = nullptr;
+	mtz_job *dec_gz = nullptr;                          // DECOMPRESS with MTZ_FLAG_GZIP_WIRE: k_inflate's jobs (k_plan_jobs)
 	mtz_rec *out_recs = nullptr;
 	RecSums *osums = nullptr;
 	StampStep *steps = nullptr;                         // per-record transitions of the stamp chain

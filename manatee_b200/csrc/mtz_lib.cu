@@ -314,6 +314,10 @@ int32_t mtz_open(const mtz_config *cfg, mtz_handle **out)
 		return fail(nullptr, MTZ_EINVAL, "BLOCK_LOGICAL extends the block check: it needs BLOCK_CKSUM");
 	if ((full.flags & MTZ_FLAG_GZIP_IN) && !(full.flags & MTZ_FLAG_COMPRESSED_IN))
 		return fail(nullptr, MTZ_EINVAL, "GZIP_IN extends COMPRESSED_IN: it needs COMPRESSED_IN");
+	if ((full.flags & MTZ_FLAG_GZIP_WIRE) && (full.flags & MTZ_FLAG_GZIP_IN))
+		return fail(nullptr, MTZ_EINVAL, "GZIP_WIRE forwards the gzip records GZIP_IN inflates: set one of them");
+	if ((full.flags & MTZ_FLAG_GZIP_WIRE) && full.mode == MTZ_MODE_COMPRESS && !(full.flags & MTZ_FLAG_COMPRESSED_IN))
+		return fail(nullptr, MTZ_EINVAL, "COMPRESS: GZIP_WIRE extends COMPRESSED_IN: it needs COMPRESSED_IN");
 	const cudaDeviceProp &prop = props[0];
 
 	mtz_handle *h = new (std::nothrow) mtz_handle();
@@ -590,6 +594,7 @@ static bool block_lzjb_on(const mtz_handle *h) { return (h->cfg.flags & MTZ_FLAG
 static bool is_codec_mode(uint32_t m);
 static bool cin_on(const mtz_handle *h);
 static bool gzip_on(const mtz_handle *h);
+static bool gzwire_on(const mtz_handle *h);
 // COMPRESS / DECOMPRESS / RECOMPRESS with MTZ_FLAG_BLOCK_LOGICAL: the block check runs jobs over the
 // logical bytes (launch_block_logical); VERIFY accepts the flag and does not change
 static bool block_logical_on(const mtz_handle *h)
@@ -603,7 +608,7 @@ static uint32_t block_fcodecs(const mtz_handle *h)
 {
 	return ((h->cfg.flags & MTZ_FLAG_BLOCK_FRAMES) && h->cfg.mode == MTZ_MODE_VERIFY ? BLK_FR_LZ4 : 0u) |
 	    (block_lzjb_on(h) ? BLK_FR_LZJB : 0u) | (block_logical_on(h) ? BLK_FR_LOGICAL : 0u) |
-	    (cin_on(h) ? BLK_FR_CIN : 0u) | (gzip_on(h) ? BLK_FR_GZIP : 0u);
+	    (cin_on(h) ? BLK_FR_CIN : 0u) | (gzip_on(h) || gzwire_on(h) ? BLK_FR_GZIP : 0u);
 }
 static uint32_t block_hashed(const mtz_handle *h)
 {
@@ -810,6 +815,13 @@ static bool gzip_on(const mtz_handle *h)
 	return cin_on(h) && (h->cfg.flags & MTZ_FLAG_GZIP_IN) != 0;
 }
 
+// MTZ_FLAG_GZIP_WIRE: COMPRESS with MTZ_FLAG_COMPRESSED_IN forwards its gzip-1 .. gzip-9 records, and
+// DECOMPRESS inflates them (k_inflate over cb.dec_gz); the other modes accept the flag and do not change
+static bool gzwire_on(const mtz_handle *h)
+{
+	return (cin_on(h) || h->cfg.mode == MTZ_MODE_DECOMPRESS) && (h->cfg.flags & MTZ_FLAG_GZIP_WIRE) != 0;
+}
+
 // K3h's hash tables: one per warp of its persistent grid (launch_k3h)
 static size_t hc_tab_bytes(const mtz_handle *h)
 {
@@ -824,6 +836,7 @@ static int32_t codec_alloc(mtz_handle *h, CodecBufs &cb, size_t rec_cap, size_t 
 	MTZ_CU(h, cudaMalloc(&cb.offs, rec_cap * sizeof(uint64_t)));
 	MTZ_CU(h, cudaMalloc(&cb.out_offs, rec_cap * sizeof(uint64_t)));
 	MTZ_CU(h, cudaMalloc(&cb.dec, rec_cap * sizeof(mtz_job)));
+	if (gzwire_on(h) && h->cfg.mode == MTZ_MODE_DECOMPRESS) MTZ_CU(h, cudaMalloc(&cb.dec_gz, rec_cap * sizeof(mtz_job)));
 	MTZ_CU(h, cudaMalloc(&cb.enc, rec_cap * sizeof(mtz_job)));
 	MTZ_CU(h, cudaMalloc(&cb.out_recs, rec_cap * sizeof(mtz_rec)));
 	MTZ_CU(h, cudaMalloc(&cb.osums, rec_cap * sizeof(RecSums)));
@@ -858,7 +871,7 @@ static int32_t codec_alloc(mtz_handle *h, CodecBufs &cb, size_t rec_cap, size_t 
 static void codec_free(CodecBufs &cb)
 {
 	cudaFree(cb.cr); cudaFree(cb.vals); cudaFree(cb.offs); cudaFree(cb.out_offs);
-	cudaFree(cb.dec); cudaFree(cb.enc); cudaFree(cb.out_recs); cudaFree(cb.osums); cudaFree(cb.steps);
+	cudaFree(cb.dec); cudaFree(cb.dec_gz); cudaFree(cb.enc); cudaFree(cb.out_recs); cudaFree(cb.osums); cudaFree(cb.steps);
 	cudaFree(cb.d_logical); cudaFree(cb.d_enc); cudaFree(cb.d_cres); cudaFree(cb.d_ores);
 	cudaFree(cb.d_outpos); cudaFree(cb.seq_n); cudaFree(cb.cert); cudaFree(cb.k3_skip); cudaFree(cb.hc_tab);
 	cudaFree(cb.chk); cudaFree(cb.chk_sums); cudaFree(cb.d_chk); cudaFree(cb.chk_pos);
@@ -911,7 +924,8 @@ static int32_t codec_launch_pre(mtz_handle *h, cudaStream_t st, CodecBufs &cb, c
 
 // plan + K2 (decode) of one (sub-)batch; in COMPRESS with MTZ_FLAG_COMPRESSED_IN the lzjb and zle
 // decoders, and with MTZ_FLAG_GZIP_IN k_inflate, in K2's place (every decode job of that mode is one
-// of theirs)
+// of theirs); in DECOMPRESS with MTZ_FLAG_GZIP_WIRE k_inflate after K2, over the gzip jobs that
+// k_plan_jobs kept out of K2's table
 static int32_t codec_launch_dec(mtz_handle *h, cudaStream_t st, CodecBufs &cb, const uint8_t *d_in,
     const mtz_rec *d_recs, size_t nrec)
 {
@@ -919,14 +933,21 @@ static int32_t codec_launch_dec(mtz_handle *h, cudaStream_t st, CodecBufs &cb, c
 	if (nrec > cb.rec_cap) return fail(h, MTZ_ENOSPC, "codec batch of %zu records exceeds %zu", nrec, cb.rec_cap);
 	const uint32_t n = (uint32_t)nrec, mode = h->cfg.mode;
 	const unsigned tb = 256, gb = (n + tb - 1) / tb;
-	k_plan_need<<<gb, tb, 0, st>>>(d_recs, n, mode, cb.cr, cb.vals, cin_on(h), gzip_on(h));
+	k_plan_need<<<gb, tb, 0, st>>>(d_recs, n, mode, cb.cr, cb.vals, cin_on(h), gzip_on(h), gzwire_on(h));
 	k_xscan_u64<<<1, XSCAN_THREADS, 0, st>>>(cb.vals, cb.offs, n, nullptr, nullptr);
-	k_plan_jobs<<<gb, tb, 0, st>>>(d_in, d_recs, n, cb.cr, cb.offs, cb.d_logical, cb.d_enc, cb.dec, cb.enc);
+	k_plan_jobs<<<gb, tb, 0, st>>>(d_in, d_recs, n, cb.cr, cb.offs, cb.d_logical, cb.d_enc, cb.dec, cb.enc,
+	    cb.dec_gz);
 	MTZ_CU(h, cudaGetLastError());
 	count_launch(h, 3);
 	if (mode != MTZ_MODE_COMPRESS) {
 		int32_t rc = launch_k2(h, st, nullptr, nullptr, cb.dec, n, cb.seq_n ? cb.enc : nullptr, cb.seq_n);
 		if (rc != MTZ_OK) return rc;
+		if (cb.dec_gz != nullptr) {
+			const unsigned gi = (unsigned)std::min<size_t>((nrec + INFL_WARPS - 1) / INFL_WARPS, (size_t)h->sm_count * 8);
+			k_inflate<<<gi, INFL_THREADS, 0, st>>>(d_recs, cb.dec_gz, n);
+			MTZ_CU(h, cudaGetLastError());
+			count_launch(h, 1);
+		}
 	} else if (cin_on(h)) {
 		const unsigned gl = (unsigned)std::min<size_t>((nrec + LZJB_WARPS - 1) / LZJB_WARPS, (size_t)h->sm_count * 8);
 		k_lzjb_decode<<<gl, LZJB_THREADS, 0, st>>>(d_recs, cb.dec, n);
@@ -983,7 +1004,7 @@ static int32_t codec_launch_post(mtz_handle *h, cudaStream_t st, CodecBufs &cb, 
 	RecSums *osums = all_osums ? all_osums + rec_base : cb.osums;
 	const uint32_t n = (uint32_t)nrec, mode = h->cfg.mode;
 	const unsigned tb = 256, gb = (n + tb - 1) / tb;
-	k_layout<<<gb, tb, 0, st>>>(d_recs, n, cb.cr, cb.dec, cb.enc, cb.vals, cb.d_cres, rec_base, cb.cert);
+	k_layout<<<gb, tb, 0, st>>>(d_recs, n, cb.cr, cb.dec, cb.enc, cb.vals, cb.d_cres, rec_base, cb.cert, cb.dec_gz);
 	k_xscan_u64<<<1, XSCAN_THREADS, 0, st>>>(cb.vals, cb.out_offs, n, cb.d_outpos, cb.d_outpos);
 	const unsigned ga = (unsigned)std::min<size_t>((n + 7) / 8, (size_t)h->sm_count * 8);
 	k_assemble<<<ga, ASM_THREADS, 0, st>>>(d_in, d_recs, n, mode, cb.cr, cb.out_offs, cb.enc,
@@ -1495,6 +1516,7 @@ static int32_t dev_finish_impl(mtz_handle *h, const uint64_t carry_in[4], const 
 		h->cstats.lzjb_decoded += c.n_lzjb;
 		h->cstats.zle_decoded += c.n_zle;
 		h->cstats.gzip_decoded += c.n_gzip;
+		h->cstats.gzip_passed += c.n_gzpass;
 	}
 	if (out_bytes) *out_bytes = ob;
 	rc = account_result(h, r, h->dv_first, h->dv_nrec, h->dv_in_bytes, ob, block_on(h) ? &h->bpend : nullptr);
@@ -1554,11 +1576,13 @@ static void wire_preamble(uint8_t out[WIRE_PRE_BYTES], uint32_t flags)
 }
 
 // 1: a preamble this side speaks (flags out); 0: not a preamble; <0: a preamble of a version or
-// with capability bits this side does not know
-static int wire_parse(const uint8_t *p, uint32_t *flags)
+// with capability bits this side does not know.  WIRE_F_GZIP is known only to a DECOMPRESS opened with
+// MTZ_FLAG_GZIP_WIRE: any other receiver refuses the wire rather than hand gzip records on.
+static int wire_parse(const mtz_handle *h, const uint8_t *p, uint32_t *flags)
 {
+	const uint32_t known = WIRE_F_ORIG_LZ4 | (gzwire_on(h) ? WIRE_F_GZIP : 0u);
 	if (rd64(p) != WIRE_MAGIC) return 0;
-	if (rd32(p + 8) != WIRE_VERSION || (rd32(p + 12) & ~WIRE_F_ORIG_LZ4) != 0) return -1;
+	if (rd32(p + 8) != WIRE_VERSION || (rd32(p + 12) & ~known) != 0) return -1;
 	for (unsigned k = 16; k < WIRE_PRE_BYTES; k++) if (p[k] != 0) return -1;
 	*flags = rd32(p + 12);
 	return 1;
@@ -1599,7 +1623,7 @@ static int32_t batch_accept(mtz_handle *h, const Slot &s, BatchCut &bc, const ui
 			// the lz4-stage-v1 wire puts a preamble in front of every BEGIN: BEGIN opens its batch
 			if (bc.cnt > 0) return 0;
 			bc.emit_pre = true;
-			bc.pre_flags = wire_orig_lz4(feat);
+			bc.pre_flags = wire_orig_lz4(feat) | (gzwire_on(h) ? WIRE_F_GZIP : 0u);
 		} else if (h->cfg.mode == MTZ_MODE_DECOMPRESS) {
 			if (!ws->pre_seen)
 				return fail(h, MTZ_EINVAL, "DECOMPRESS: stream was not produced by the COMPRESS stage");
@@ -1672,6 +1696,7 @@ static int32_t harvest(mtz_handle *h, Slot &s)
 		h->cstats.lzjb_decoded += c.n_lzjb;
 		h->cstats.zle_decoded += c.n_zle;
 		h->cstats.gzip_decoded += c.n_gzip;
+		h->cstats.gzip_passed += c.n_gzpass;
 	}
 	int32_t rc = account_result(h, *s.h_res, s.first_rec, s.nrec, s.bytes, s.out_bytes,
 	    block_on(h) ? &bp : nullptr);
@@ -1866,7 +1891,7 @@ int32_t mtz_process_host(mtz_handle *h, const void *in, size_t n, void *out, siz
 				    rd64(hp) == WIRE_MAGIC) {
 					// the preamble of the lz4-stage-v1 wire: stripped here, between two batches
 					if (bc.cnt > 0) break;
-					if (wire_parse(hp, &ws.pre_flags) < 0) {
+					if (wire_parse(h, hp, &ws.pre_flags) < 0) {
 						rc = fail(h, MTZ_EFORMAT, "unsupported wire version / capability in the preamble at offset %zu", at);
 						break;
 					}

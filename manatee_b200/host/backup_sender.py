@@ -113,13 +113,20 @@ class BackupSender(object):
         receiver that looks at the job on connect sees it: the stage-compressed wire is used
         only when this sender compresses AND every requester of this send advertised
         `accept: "lz4-stage-v1"`; everybody else gets the raw (verified) stream.  With the gpu
-        stage off the job object is left exactly as the reference has it (no `wire` field)."""
+        stage off the job object is left exactly as the reference has it (no `wire` field).
+        On the stage wire with gpu.sendCompressed, `wireGzip` says whether gzip records travel as
+        their disk frames (MTZ_FLAG_GZIP_WIRE): only when every requester also advertised
+        `acceptGzip: true`, since the receiver's stage then inflates them."""
         if not self._gpu or self._gpu.get("mode", "off") == "off":
             return
         compress = self._gpu["mode"] == "compress" and \
             all(j.get("accept") == "lz4-stage-v1" for j in jobs)
+        gzip_wire = compress and bool(self._gpu.get("sendCompressed")) and \
+            all(j.get("acceptGzip") is True for j in jobs)
         for j in jobs:
             j["wire"] = "lz4-stage-v1" if compress else "raw"
+            if compress and self._gpu.get("sendCompressed"):
+                j["wireGzip"] = gzip_wire
 
     def _send_compressed(self, backupJob):
         """`zfs send -c` for this job: gpu.sendCompressed is set and _decide_wire chose the stage wire"""
@@ -144,12 +151,14 @@ class BackupSender(object):
                                 block_logical=bool(g.get("blockLogical")),
                                 lz4_hc=bool(g.get("lz4Hc")),
                                 compressed_input=self._send_compressed(backupJob),
-                                gzip_input=self._send_compressed(backupJob) and bool(g.get("sendGzip")))
+                                gzip_input=self._send_compressed(backupJob) and bool(g.get("sendGzip"))
+                                and not backupJob.get("wireGzip"),
+                                gzip_wire=self._send_compressed(backupJob) and bool(backupJob.get("wireGzip")))
 
     def _stage_stats(self, stage):
         """job.gpu: the stage counters, plus `blocks` (block-checksum counters) with
         gpu.blockChecksums set and `compressed_in` (mtz_get_compressed_in_stats) with gpu.sendCompressed,
-        gzip_decoded included with gpu.sendGzip"""
+        gzip_decoded included with gpu.sendGzip, gzip_passed on a `wireGzip` job"""
         st = stage.stats()
         if self._gpu.get("blockChecksums"):
             st["blocks"] = stage.block_stats()
@@ -237,8 +246,8 @@ class BackupSender(object):
                 self._decide_wire([backupJob])
                 sock = socket.create_connection((backupJob["host"], int(backupJob["port"])))
             # gpu.sendCompressed: a compressed-wire job takes the disk frames (`zfs send -c`), which the
-            # COMPRESS stage forwards (LZ4) or decodes and re-encodes (lzjb / zle, and gzip with
-            # gpu.sendGzip); every other job
+            # COMPRESS stage forwards (LZ4, and gzip on a `wireGzip` job) or decodes and re-encodes
+            # (lzjb / zle, and gzip with gpu.sendGzip); every other job
             # spawns the reference's command
             flags = ["-c"] if self._send_compressed(backupJob) else []
             zfsSend = subprocess.Popen([self._zfsPath, "send"] + flags + ["-v", "-P", snapshot],

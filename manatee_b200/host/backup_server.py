@@ -104,6 +104,8 @@ class BackupServer(object):
                        "dataset": params["dataset"], "done": False}
                 if params.get("accept"):
                     job["accept"] = params["accept"]      # wire capability of the receiver (f2)
+                if params.get("acceptGzip") in (True, "true"):
+                    job["acceptGzip"] = True              # ... and gzip frames on that wire
                 self._send(200, {"jobid": job["uuid"], "jobPath": "/backup/" + job["uuid"]})
                 queue.push(job)
 

@@ -117,7 +117,10 @@ class ZfsClient(object):
             return None
         from ..stage import GpuSnapshotStage
         g = self._gpu
+        # gpu.acceptGzip: a DECOMPRESS stage that inflates the gzip frames a sender forwards
+        # (MTZ_FLAG_GZIP_WIRE); it decodes an ordinary lz4-stage-v1 wire exactly as without the flag
         return GpuSnapshotStage(mode or g["mode"], device=g.get("device", 0),
+                                gzip_wire=(mode or g["mode"]) == "decompress" and bool(g.get("acceptGzip")),
                                 ring_bytes=g.get("ringBytes", 0), batch_bytes=g.get("batchBytes", 0),
                                 out_ring_bytes=g.get("outRingBytes", 0), n_slots=g.get("slots", 0),
                                 block_checksums=bool(g.get("blockChecksums")),
@@ -150,6 +153,8 @@ class ZfsClient(object):
         # reference receiver never sends this, so mixed-version shards stay on the raw wire.
         if self._gpu and self._gpu.get("mode") == "decompress":
             req_body["accept"] = "lz4-stage-v1"
+            if self._gpu.get("acceptGzip"):
+                req_body["acceptGzip"] = True             # this stage inflates gzip frames on the GPU
         body = json.dumps(req_body).encode()
         req = urllib.request.Request(serverUrl.rstrip("/") + "/backup", data=body,
                                      headers={"Content-Type": "application/json"})

@@ -22,7 +22,7 @@ class GpuSnapshotStage(object):
     def __init__(self, mode="verify", device=0, ring_bytes=0, batch_bytes=0, n_slots=0,
                  out_ring_bytes=0, flags=0, devices=None, block_checksums=False, block_sha256=False,
                  block_sha512=False, block_frames=False, block_lzjb=False, block_logical=False,
-                 lz4_hc=False, compressed_input=False, gzip_input=False):
+                 lz4_hc=False, compressed_input=False, gzip_input=False, gzip_wire=False):
         """``devices`` = CUDA ordinals of a device group: the GPUs of one box run as ONE stage,
         batch b of the stream on ``devices[b % len(devices)]`` (mtz_config.devices[]).
         ``block_checksums`` = MTZ_FLAG_BLOCK_CKSUM: every DRR_WRITE is also checked against the
@@ -57,7 +57,14 @@ class GpuSnapshotStage(object):
         ``gzip_input`` = MTZ_FLAG_GZIP_IN, only valid with ``compressed_input``: COMPRESS also inflates
         the gzip-1 .. gzip-9 records on the GPU and encodes them like raw ones; a frame zlib would not
         inflate to exactly drr_logical_size bytes is ECODEC.  ``compressed_in_stats()`` then also
-        reports ``gzip_decoded``.  The other modes accept it and do not change."""
+        reports ``gzip_decoded``.  The other modes accept it and do not change.
+        ``gzip_wire`` = MTZ_FLAG_GZIP_WIRE, gzip frames on the compressed wire; never with ``gzip_input``.
+        COMPRESS (only valid with ``compressed_input``) forwards the gzip-1 .. gzip-9 records as they are
+        and marks every wire preamble with the gzip capability bit (``compressed_in_stats()`` then also
+        reports ``gzip_passed``).  DECOMPRESS accepts that bit, inflates the gzip records on the GPU by
+        ``gzip_input``'s rule and writes them raw, as plain `zfs send` would have (``gzip_decoded``); a
+        DECOMPRESS stage without it refuses such a wire with EFORMAT.  The other modes accept it and do
+        not change."""
         if block_checksums:
             flags |= N.FLAG_BLOCK_CKSUM
         if block_sha256:
@@ -76,7 +83,10 @@ class GpuSnapshotStage(object):
             flags |= N.FLAG_COMPRESSED_IN
         if gzip_input:
             flags |= N.FLAG_GZIP_IN
+        if gzip_wire:
+            flags |= N.FLAG_GZIP_WIRE
         self._gzip_input = bool(gzip_input)
+        self._gzip_wire = bool(gzip_wire)
         self._L = N.lib()
         self._h = C.c_void_p()
         cfg = N.Config()
@@ -140,14 +150,17 @@ class GpuSnapshotStage(object):
 
     def compressed_in_stats(self):
         """MTZ_FLAG_COMPRESSED_IN counters (mtz_get_compressed_in_stats): lz4_passed, lzjb_decoded,
-        zle_decoded, and gzip_decoded for a stage opened with ``gzip_input``; all zero without
-        ``compressed_input``."""
+        zle_decoded, gzip_decoded for a stage opened with ``gzip_input`` or ``gzip_wire``, and gzip_passed
+        for one opened with ``gzip_wire``; all zero without ``compressed_input`` (DECOMPRESS with
+        ``gzip_wire`` counts gzip_decoded)."""
         st = N.CompressedInStats()
         st.struct_size = C.sizeof(N.CompressedInStats)
         self._check(self._L.mtz_get_compressed_in_stats(self._h, C.byref(st)))
         d = st.as_dict()
-        if not self._gzip_input:
+        if not (self._gzip_input or self._gzip_wire):
             del d["gzip_decoded"]
+        if not self._gzip_wire:
+            del d["gzip_passed"]
         return d
 
     def end_checksum(self):

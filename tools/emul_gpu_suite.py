@@ -54,6 +54,7 @@ PARAMS = {
     "test_block_counters_are_those_of_verify": [(False,), (True,)],
     "test_inflated_output_equals_the_model": [("gzip-1", 8192), ("gzip-6", 8192), ("gzip-9", 8192), ("mixed", 8192)],
     "test_gzip_block_counters": [(False, False), (True, True)],
+    "test_round_trip_equals_the_model": [("gzip-1", 8192), ("gzip-6", 8192), ("gzip-9", 8192), ("mixed", 8192)],
 }
 SKIP = {"test_sixteen_mib_record": "16 MiB blocks take minutes per encode on the emulator",
         "test_size_independent_properties_at_2gib": "2 GiB of LZ4 work is out of reach for the emulator",
@@ -88,12 +89,13 @@ def main():
     import test_gpu_codec as K
     import test_gpu_compressed_in as CI
     import test_gpu_gzip_in as GZ
+    import test_gpu_gzip_wire as GW
     import test_gpu_lz4 as Z
     import test_gpu_lz4hc as HC
     import test_gpu_stream as S
     import test_gpu_verify as V
     tot = fail = 0
-    for mod in (V, S, Z, K, B, H, W, F, J, L, HC, CI, GZ):
+    for mod in (V, S, Z, K, B, H, W, F, J, L, HC, CI, GZ, GW):
         for name, fn in inspect.getmembers(mod, inspect.isfunction):
             if not name.startswith("test_") or filt not in name:
                 continue

@@ -30,6 +30,12 @@ power limit and max SM clock the numbers were taken on.
   gzip_in        MTZ_FLAG_GZIP_IN: the same legs, the flag leg with compressed_input + gzip_input, for
                  pg-page 128 KiB records written with gzip-1, gzip-6, gzip-9 and a gzip-6 / lz4 / lzjb /
                  raw pool; plus k_inflate's device time and single-thread zlib.decompress of the records
+  gzip_wire      MTZ_FLAG_GZIP_WIRE on the pools of gzip_in.  Sender: COMPRESS of x with compressed_input +
+                 gzip_input (today's wire) against compressed_input + gzip_wire: wire bytes, resident step,
+                 mtz_process_host and the ring API through a pipe.  Receiver: DECOMPRESS of today's wire
+                 against DECOMPRESS with gzip_wire of the gzip wire, and DECOMPRESS with gzip_wire of today's
+                 wire (no gzip record on it): resident step, mtz_process_host, k_inflate and K2 device time;
+                 every DECOMPRESS output is checked against plain(x); --pools picks some of the pools
 
 A resident step is timed with CUDA events around dev_submit + dev_finish on a side stream, a host pass
 with the host clock around mtz_process_host; kernel device times come from torch.profiler in a pass of
@@ -53,6 +59,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import block_ref as R  # noqa: E402
 import compressed_in_ref as CI  # noqa: E402
 import gzip_in_ref as GZ  # noqa: E402
+import gzip_wire_ref as GW  # noqa: E402
 import oracle as O  # noqa: E402
 
 RECSIZE = 131072
@@ -507,6 +514,131 @@ def gzip_in(a):
                        ("k_inflate", "k_lzjb_decode", "k3_lz4_encode"), zlib_rate)
 
 
+def dev_legs(a, legs, logical, profile=None, kernels=()):
+    """resident steps of `legs` {name: (mode, GpuSnapshotStage keyword arguments, input stream)}, alternating:
+    ms per dev_submit + dev_finish (CUDA events on a side stream), output bytes and the output of the last
+    step per leg; with `profile` that leg's `kernels` device time (a pass of its own)"""
+    import numpy as np
+    import torch
+    from manatee_b200 import GpuSnapshotStage, index_host
+    bufs = {}
+    for n, (_, _, src) in legs.items():
+        recs, _ = index_host(src)
+        cap = int(np.maximum(recs["lsize"], recs["payload"]).sum()) + 312 * len(recs) + (1 << 20)
+        bufs[n] = (torch.from_numpy(src).cuda(), torch.from_numpy(recs.view(np.uint8).copy()).cuda(), len(recs),
+                   torch.empty(cap, dtype=torch.uint8, device="cuda"), cap)
+    st = torch.cuda.Stream()
+    ms, nout, outs = {n: [] for n in legs}, {}, {}
+    with ExitStack() as es:
+        gs = {n: es.enter_context(GpuSnapshotStage(mode, **kw)) for n, (mode, kw, _) in legs.items()}
+
+        def step(n):
+            g, (d_in, d_recs, nrec, d_out, cap) = gs[n], bufs[n]
+            g.dev_reset()
+            torch.cuda.synchronize()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(st)
+            g.dev_submit(d_in.data_ptr(), d_in.numel(), d_recs.data_ptr(), nrec, d_out.data_ptr(), cap,
+                         cuda_stream=st.cuda_stream)
+            ob = g.dev_finish()[0]
+            e1.record(st)
+            torch.cuda.synchronize()
+            return e0.elapsed_time(e1), ob
+
+        for i, n in alternate(legs, a.warmup + a.steps):
+            t, ob = step(n)
+            if i >= a.warmup:
+                ms[n].append(t)
+            nout[n] = int(ob)
+        for n in legs:
+            outs[n] = bufs[n][3][:nout[n]].cpu().numpy()
+        names = list(legs)
+        res = {}
+        for k in range(1, len(names)):
+            res.update(summary((names[0], names[k]), ms, logical, "logical_gbps"))
+            res[names[k] + "_diff_ms_mean"] = res.pop("diff_ms_mean")
+            res[names[k] + "_diff_pct_mean"] = res.pop("diff_pct_mean")
+        res.update({n + "_out_bytes": nout[n] for n in names})
+        res["compressed_in_stats"] = {n: gs[n].compressed_in_stats() for n in names}
+        res["lz4_decoded"] = {n: gs[n].stats()["lz4_decoded"] for n in names}
+        if profile is not None and a.profile_steps:
+            res[profile + "_kernels"] = kernel_times(partial(step, profile), a.profile_steps, kernels)
+    del bufs
+    torch.cuda.empty_cache()
+    return res, outs
+
+
+def host_legs(a, legs, logical):
+    """wall ms per mtz_process_host pass of `legs` (as dev_legs), 1 warm-up and --host-steps timed,
+    alternating; the output of each leg's last pass"""
+    import numpy as np
+    from manatee_b200 import GpuSnapshotStage
+    hms, outs = {n: [] for n in legs}, {}
+    with ExitStack() as es:
+        gs = {n: es.enter_context(GpuSnapshotStage(mode, **kw)) for n, (mode, kw, _) in legs.items()}
+        for i, n in alternate(legs, 1 + a.host_steps):
+            src = legs[n][2]
+            out = np.zeros(src.size * 4 + (64 << 20), dtype=np.uint8)
+            t0 = time.perf_counter()
+            ob = gs[n].process_host(src, out)
+            if i >= 1:
+                hms[n].append((time.perf_counter() - t0) * 1e3)
+            outs[n] = out[:ob].copy()
+            del out
+    names = list(legs)
+    res = {}
+    for k in range(1, len(names)):
+        res.update(summary((names[0], names[k]), hms, logical, "logical_gbps"))
+        res[names[k] + "_diff_ms_mean"] = res.pop("diff_ms_mean")
+        res[names[k] + "_diff_pct_mean"] = res.pop("diff_pct_mean")
+    return res, outs
+
+
+def gzip_wire(a):
+    """the sender and the receiver of MTZ_FLAG_GZIP_WIRE on the pools of gzip_in (module docstring)"""
+    import numpy as np
+    import bench
+    from manatee_b200 import GpuSnapshotStage, index_host
+    today = {"compressed_input": True, "gzip_input": True}
+    flag = {"compressed_input": True, "gzip_wire": True}
+    res = {"payload": "pg-page 128 KiB records (oracle.gen_payload(PAYLOAD_PGPAGE, r, 131072))"}
+    for sname, codec, ashift in GZIP_STREAMS:
+        if sname not in a.pools.split(","):
+            continue
+        p = keyed(O, synth(a.gib, O.PAYLOAD_PGPAGE), NTH, codec, ashift)
+        x = GZ.as_send_c(O, p, ashift)
+        logical = int(index_host(p)[0]["lsize"].sum())
+        r = {"logical_bytes": logical, "plain_bytes": int(p.size), "send_c_bytes": int(x.size),
+             "gzip_records": sum(1 for _, off, _, _ in CI.write_records(x) if GZ.is_gzip(int(x[off + 50])))}
+        send = {"lz4_wire": ("compress", today, x), "gzip_wire": ("compress", flag, x)}
+        r["sender_resident"], _ = dev_legs(a, send, logical)
+        r["sender_host"], wires = host_legs(a, send, logical)
+        r["lz4_wire_bytes"], r["gzip_wire_bytes"] = int(wires["lz4_wire"].size), int(wires["gzip_wire"].size)
+        r["wire_saving_pct"] = 100.0 * (1 - r["gzip_wire_bytes"] / r["lz4_wire_bytes"])
+        r["gzip_wire_equals_the_model"] = bool(np.array_equal(wires["gzip_wire"], GW.splice(O, wires["lz4_wire"], x)))
+        secs = {n: [] for n in send}
+        for _, n in alternate(send, a.ring_steps):
+            with GpuSnapshotStage("compress", **send[n][1]) as g:
+                dt, ok, detail = bench.ring_run(g, x, producer="pipe")
+                assert ok, detail
+                secs[n].append(dt)
+        r["sender_ring_pipe"] = {n + "_logical_gbps_mean": logical / (sum(v) / len(v)) / 1e9 for n, v in secs.items()}
+        # the receiver: the device API takes the wire without its preambles
+        want = GZ.plain(O, x)
+        lzw, gzw = wires["lz4_wire"], wires["gzip_wire"]
+        recv = {"lz4_wire": ("decompress", {}, O.wire_strip(lzw)), "gzip_wire": ("decompress", {"gzip_wire": True},
+                O.wire_strip(gzw)), "flag_on_lz4_wire": ("decompress", {"gzip_wire": True}, O.wire_strip(lzw))}
+        r["receiver_resident"], outs = dev_legs(a, recv, logical, "gzip_wire", ("k_inflate", "k2_lz4_decode"))
+        recv_host = {n: (m, kw, {"lz4_wire": lzw, "gzip_wire": gzw, "flag_on_lz4_wire": lzw}[n])
+                     for n, (m, kw, _) in recv.items()}
+        r["receiver_host"], houts = host_legs(a, recv_host, logical)
+        r["decompressed_equals_plain"] = {n: bool(np.array_equal(houts[n], want)) for n in recv}
+        r["resident_decompressed_equals_plain"] = {n: bool(np.array_equal(outs[n], want)) for n in recv}
+        res[sname] = r
+        del p, x, wires, outs, houts
+    return res
+
+
 SHA_OPTIONS = dict(verify_gib=16.0, host_gib=2.0, recompress_gib=1.0, steps=10, warmup=2, host_steps=4,
                    profile_steps=3)
 FRAME_OPTIONS = dict(verify_gib=16.0, host_gib=2.0, ring_gib=8.0, steps=10, warmup=2, host_steps=4, ring_steps=3,
@@ -523,6 +655,8 @@ WORKLOADS = {
     "lz4hc": (lz4hc, dict(gib=1.0, host_gib=1.0, steps=5, warmup=1, host_steps=3, profile_steps=2)),
     "compressed_in": (compressed_in, dict(gib=0.5, steps=5, warmup=1, host_steps=3, ring_steps=3, profile_steps=2)),
     "gzip_in": (gzip_in, dict(gib=0.5, steps=5, warmup=1, host_steps=3, ring_steps=3, profile_steps=2)),
+    "gzip_wire": (gzip_wire, dict(gib=0.5, steps=5, warmup=1, host_steps=3, ring_steps=3, profile_steps=2,
+                                  pools=",".join(s[0] for s in GZIP_STREAMS))),
 }
 
 
