@@ -182,6 +182,30 @@ extern "C" {
                                   * .gzip_passed (COMPRESS) and .gzip_decoded (DECOMPRESS).  VERIFY,
                                   * RECOMPRESS and PASSTHROUGH accept the flag and do not change */
 
+#define MTZ_FLAG_GZIP_ENCODE 4096u /* COMPRESS: deflate on the compressed wire.  Never with MTZ_FLAG_LZ4_HC
+                                  * or MTZ_FLAG_GZIP_IN (MTZ_EINVAL; forward gzip input with
+                                  * MTZ_FLAG_GZIP_WIRE, which this flag combines with).  Each DRR_WRITE that
+                                  * K3 stores as an LZ4 frame (a raw record, and with MTZ_FLAG_COMPRESSED_IN
+                                  * a decoded lzjb / zle one) is also re-coded from K3's parse as one
+                                  * dynamic-Huffman deflate block in a zlib stream (CMF 0x78, FLG 0x01,
+                                  * Adler-32 trailer) zero-padded to a multiple of 512 bytes (DESIGN.md
+                                  * section 1 defines the frame); when that is strictly smaller than the
+                                  * LZ4 frame the record leaves with it, drr_compressiontype 5 (gzip-1) and
+                                  * drr_compressed_size the padded size.  No record gets larger than without
+                                  * the flag; a record K3 stores raw stays raw; LZ4 (and with
+                                  * MTZ_FLAG_GZIP_WIRE gzip) input records are forwarded as before.  Every
+                                  * wire preamble carries WIRE_F_GZIP (2), so only a DECOMPRESS opened with
+                                  * MTZ_FLAG_GZIP_WIRE accepts the wire (any other: MTZ_EFORMAT).  With
+                                  * MTZ_FLAG_BLOCK_CKSUM a raw record with an LZ4 key that leaves as gzip is
+                                  * compared with its output (frame_miss, never an error).  Counters:
+                                  * mtz_compressed_in_stats.gzip_encoded counts the gzip records and
+                                  * mtz_stats.lz4_encoded only the LZ4 ones (their sum is lz4_encoded
+                                  * without the flag).  Device memory: one more job table (32 B a record)
+                                  * and one more frame scratch as large as the encoder's per codec batch
+                                  * in flight (n_slots x devices of them for the ring API and
+                                  * mtz_process_host, two for the device API).  VERIFY, DECOMPRESS,
+                                  * RECOMPRESS and PASSTHROUGH accept the flag and do not change */
+
 typedef struct mtz_handle mtz_handle;
 
 #define MTZ_MAX_DEVICES 16
@@ -264,6 +288,8 @@ typedef struct mtz_compressed_in_stats {
 	                               the GPU; likewise in DECOMPRESS with MTZ_FLAG_GZIP_WIRE */
 	uint64_t gzip_passed;       /* COMPRESS with MTZ_FLAG_GZIP_WIRE: ... that arrived gzip-1 .. gzip-9 and
 	                               were forwarded as they are */
+	uint64_t gzip_encoded;      /* COMPRESS with MTZ_FLAG_GZIP_ENCODE: DRR_WRITEs that left as the stage's
+	                               gzip-1 frame (with or without MTZ_FLAG_COMPRESSED_IN) */
 } mtz_compressed_in_stats;
 
 /* One DRR record as seen by the kernels (32 B, little endian). */
@@ -435,6 +461,13 @@ int32_t mtz_k_lz4_encode(mtz_handle *h, const void *d_src, void *d_dst,
 /* the MTZ_FLAG_LZ4_HC encoder (K3h) on any handle, same contract as mtz_k_lz4_encode; its hash
  * tables (132 MiB on a 132-SM H100) are allocated on the first call and freed by mtz_close */
 int32_t mtz_k_lz4hc_encode(mtz_handle *h, const void *d_src, void *d_dst,
+    mtz_job *d_jobs, uint32_t njobs, void *cuda_stream);
+/* the MTZ_FLAG_GZIP_ENCODE encoder on any handle, mtz_k_lz4_encode's contract: K3, then the deflate
+ * re-coding of its frame.  out_len = the padded size of the zlib frame written to the slot when K3
+ * makes an LZ4 frame and the zlib frame is smaller than lsize, else lsize (store raw).  d_dst and every
+ * dst_off must be 4-byte aligned (MTZ_EINVAL).  It reads the job table to size a scratch for K3's
+ * frames (kept by the handle, freed by mtz_close), so it synchronises the stream */
+int32_t mtz_k_gzip_encode(mtz_handle *h, const void *d_src, void *d_dst,
     mtz_job *d_jobs, uint32_t njobs, void *cuda_stream);
 
 #ifdef __cplusplus

@@ -27,6 +27,7 @@ FLAG_LZ4_HC = 256
 FLAG_COMPRESSED_IN = 512
 FLAG_GZIP_IN = 1024
 FLAG_GZIP_WIRE = 2048
+FLAG_GZIP_ENCODE = 4096
 XCHG_FIRST, XCHG_LAST = 1, 2
 MODE_NAMES = {"verify": 0, "compress": 1, "decompress": 2, "recompress": 3, "passthrough": 4}
 
@@ -72,7 +73,7 @@ class BlockStats(C.Structure):
 class CompressedInStats(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("pad", C.c_uint32), ("lz4_passed", C.c_uint64),
                 ("lzjb_decoded", C.c_uint64), ("zle_decoded", C.c_uint64), ("gzip_decoded", C.c_uint64),
-                ("gzip_passed", C.c_uint64)]
+                ("gzip_passed", C.c_uint64), ("gzip_encoded", C.c_uint64)]
 
     def as_dict(self):
         return {k: getattr(self, k) for k, _ in self._fields_[2:]}
@@ -91,7 +92,7 @@ SYMBOLS = [
     "mtz_get_block_stats", "mtz_get_compressed_in_stats", "mtz_end_checksum", "mtz_host_alloc", "mtz_host_free", "mtz_process_host",
     "mtz_index_host", "mtz_dev_index", "mtz_dev_submit", "mtz_dev_aggregate",
     "mtz_dev_finish", "mtz_dev_reset", "mtz_dev_aggregate_async", "mtz_dev_finish_gathered", "mtz_set_carry",
-    "mtz_k_lz4_decode", "mtz_k_lz4_encode", "mtz_k_lz4hc_encode",
+    "mtz_k_lz4_decode", "mtz_k_lz4_encode", "mtz_k_lz4hc_encode", "mtz_k_gzip_encode",
     "mtz_fanout_attach", "mtz_out_peek_peer", "mtz_out_consume_peer", "mtz_read_peer", "mtz_cancel",
     "mtz_comm_unique_id", "mtz_comm_init", "mtz_comm_share", "mtz_dev_finish_exchange",
 ]
@@ -169,6 +170,7 @@ def lib():
     L.mtz_k_lz4_decode.argtypes = [H, vp, vp, vp, C.c_uint32, vp]
     L.mtz_k_lz4_encode.argtypes = [H, vp, vp, vp, C.c_uint32, vp]
     L.mtz_k_lz4hc_encode.argtypes = [H, vp, vp, vp, C.c_uint32, vp]
+    L.mtz_k_gzip_encode.argtypes = [H, vp, vp, vp, C.c_uint32, vp]
     for s in SYMBOLS:
         getattr(L, s).restype = getattr(L, s).restype if s in (
             "mtz_last_error", "mtz_strerror") else i32

@@ -35,8 +35,9 @@ namespace mtz {
 #define WIRE_VERSION    1u
 #define WIRE_PRE_BYTES  32u
 #define WIRE_F_ORIG_LZ4 1u
-#define WIRE_F_GZIP     2u      // COMPRESS with MTZ_FLAG_GZIP_WIRE: gzip frames may follow.  Only a DECOMPRESS
-                                // opened with that flag accepts the bit; any other refuses the preamble
+#define WIRE_F_GZIP     2u      // COMPRESS with MTZ_FLAG_GZIP_WIRE or MTZ_FLAG_GZIP_ENCODE: gzip frames may
+                                // follow.  Only a DECOMPRESS opened with MTZ_FLAG_GZIP_WIRE accepts the bit;
+                                // any other refuses the preamble
 #define ZIO_LZ4         15u
 
 struct CodecRec {          // 32 B per record, device only
@@ -60,7 +61,8 @@ struct CodecResult {       // device, mirrored to pinned host
 	uint32_t n_gzip;       // ... with MTZ_FLAG_GZIP_IN gzip records inflated (likewise); also DECOMPRESS
 	                       // with MTZ_FLAG_GZIP_WIRE
 	uint32_t n_gzpass;     // COMPRESS with MTZ_FLAG_GZIP_WIRE: gzip records forwarded (not in n_pass)
-	uint32_t pad;
+	uint32_t n_gz_enc;     // COMPRESS with MTZ_FLAG_GZIP_ENCODE: records stored as the stage's zlib frame
+	                       // (not in n_enc)
 };
 
 // ---- plan, step 1: flags + scratch need -----------------------------------
@@ -188,10 +190,19 @@ __global__ void k_plan_jobs(const uint8_t *__restrict__ d_in, const mtz_rec *__r
 }
 
 // ---- layout: output payload length per record -----------------------------
+// `gz_enc` (COMPRESS with MTZ_FLAG_GZIP_ENCODE): k_deflate_from_lz4's jobs; a record leaves as its zlib
+// frame (gzip-1, at gz_enc[r].dst_off) when gz_enc[r].out_len < enc[r].out_len, i.e. when that frame was
+// written.
+__device__ __forceinline__ bool gz_wins(const mtz_job *gz, const mtz_job *enc, uint32_t r)
+{
+	return gz != nullptr && gz[r].out_len < enc[r].out_len;
+}
+
 __global__ void k_layout(const mtz_rec *__restrict__ recs, uint32_t n, CodecRec *__restrict__ cr,
     const mtz_job *__restrict__ dec, const mtz_job *__restrict__ enc,
     uint64_t *__restrict__ vals, CodecResult *__restrict__ res, uint32_t rec_base,
-    const uint32_t *__restrict__ cert = nullptr, const mtz_job *__restrict__ dec_gz = nullptr)
+    const uint32_t *__restrict__ cert = nullptr, const mtz_job *__restrict__ dec_gz = nullptr,
+    const mtz_job *__restrict__ gz_enc = nullptr)
 {
 	const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
 	if (r >= n) return;
@@ -208,8 +219,9 @@ __global__ void k_layout(const mtz_rec *__restrict__ recs, uint32_t n, CodecRec 
 	}
 	if (c.flags & CF_PASS) atomicAdd(gz ? &res->n_gzpass : &res->n_pass, 1u);
 	if ((c.flags & CF_ENC) && enc[r].out_len < rec.lsize) {
-		len = enc[r].out_len;
-		atomicAdd(&res->n_enc, 1u);
+		const bool g = gz_wins(gz_enc, enc, r);
+		len = g ? gz_enc[r].out_len : enc[r].out_len;
+		atomicAdd(g ? &res->n_gz_enc : &res->n_enc, 1u);
 		if (cert != nullptr && cert[r] != 0u) atomicAdd(&res->n_cert, 1u);
 	}
 	c.out_len = len;
@@ -248,7 +260,7 @@ k_assemble(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs, u
     uint32_t mode, CodecRec *__restrict__ cr, const uint64_t *__restrict__ out_offs,
     const mtz_job *__restrict__ enc, const uint8_t *d_logical, const uint8_t *d_enc,
     uint8_t *__restrict__ d_out, mtz_rec *__restrict__ out_recs,
-    const uint32_t *__restrict__ cert = nullptr)
+    const uint32_t *__restrict__ cert = nullptr, const mtz_job *__restrict__ gz_enc = nullptr)
 {
 	const int lane = threadIdx.x & 31;
 	const uint32_t gw = blockIdx.x * (ASM_THREADS / 32) + (threadIdx.x >> 5);
@@ -268,7 +280,15 @@ k_assemble(const uint8_t *__restrict__ d_in, const mtz_rec *__restrict__ recs, u
 		uint32_t ncopy = c.out_len;
 		if (c.flags & CF_WRITE) {
 			const bool enc_ok = (c.flags & CF_ENC) && enc[r].out_len < rec.lsize;
-			if (enc_ok) {
+			if (enc_ok && gz_wins(gz_enc, enc, r)) {
+				// the stage's zlib frame, zero-padded by k_deflate_from_lz4 itself
+				psrc = reinterpret_cast<const uint8_t *>((uintptr_t)gz_enc[r].dst_off);
+				ocomp = ZIO_GZIP1;
+				if (lane == 0) {
+					hout[50] = (uint8_t)ZIO_GZIP1;
+					*reinterpret_cast<uint64_t *>(hout + 96) = (uint64_t)c.out_len;
+				}
+			} else if (enc_ok) {
 				// certified (K3c): the frame is the input's own BE32(clen) + block, zero-padded
 				const uint32_t cl = cert ? cert[r] : 0u;
 				if (cl != 0u) ncopy = cl; else psrc = d_enc + c.scratch;

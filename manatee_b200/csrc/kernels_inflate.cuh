@@ -151,6 +151,35 @@ __device__ __forceinline__ int huff_decode(InflBits &br, const uint16_t *tab, co
 	return -1;
 }
 
+// Adler-32 of [p, p+n), warp-parallel; every lane gets it
+__device__ __forceinline__ uint32_t warp_adler32(const uint8_t *p0, uint32_t n, int lane)
+{
+	const uint32_t FULL = 0xffffffffu;
+	uint64_t a = 0, b = 0;
+	auto add = [&](uint32_t p, uint32_t v) { a += v; b += (uint64_t)(n - p) * v; };
+	uint32_t tail = 0;
+	if (((uintptr_t)p0 & 15u) == 0u) {
+		tail = n & ~15u;
+		for (uint32_t p = 16u * (uint32_t)lane; p < tail; p += 512u) {
+			const uint4 v = *reinterpret_cast<const uint4 *>(p0 + p);
+			const uint32_t w[4] = { v.x, v.y, v.z, v.w };
+#pragma unroll
+			for (int q = 0; q < 16; q++) add(p + (uint32_t)q, (w[q >> 2] >> (8 * (q & 3))) & 0xffu);
+		}
+	}
+	for (uint32_t p = tail + (uint32_t)lane; p < n; p += 32u) add(p, p0[p]);
+	uint32_t sa = (uint32_t)(a % 65521u), sb = (uint32_t)(b % 65521u);
+#pragma unroll
+	for (int d = 16; d > 0; d >>= 1) {
+		sa += __shfl_xor_sync(FULL, sa, d);
+		sb += __shfl_xor_sync(FULL, sb, d);
+		sa %= 65521u; sb %= 65521u;
+	}
+	sa = (sa + 1u) % 65521u;
+	sb = (uint32_t)((sb + (uint64_t)n) % 65521u);
+	return (sb << 16) | sa;
+}
+
 // zlib's uncompress of [src, src+s_len) to exactly lsize bytes at dst: MTZ_OK or MTZ_ECODEC
 __device__ __forceinline__ int32_t warp_inflate(const uint8_t *__restrict__ src, uint32_t s_len,
     uint8_t *__restrict__ dst, uint32_t lsize, InflSmem &S, int lane)
@@ -316,29 +345,7 @@ __device__ __forceinline__ int32_t warp_inflate(const uint8_t *__restrict__ src,
 	const uint32_t want = ((t & 0xffu) << 24) | ((t >> 8) << 16) | ((t2 & 0xffu) << 8) | (t2 >> 8);
 	if (br.over() || o != lsize) return MTZ_ECODEC;
 	__syncwarp();
-	uint64_t a = 0, b = 0;
-	auto add = [&](uint32_t p, uint32_t v) { a += v; b += (uint64_t)(lsize - p) * v; };
-	uint32_t tail = 0;
-	if (((uintptr_t)dst & 15u) == 0u) {
-		tail = lsize & ~15u;
-		for (uint32_t p = 16u * (uint32_t)lane; p < tail; p += 512u) {
-			const uint4 v = *reinterpret_cast<const uint4 *>(dst + p);
-			const uint32_t w[4] = { v.x, v.y, v.z, v.w };
-#pragma unroll
-			for (int q = 0; q < 16; q++) add(p + (uint32_t)q, (w[q >> 2] >> (8 * (q & 3))) & 0xffu);
-		}
-	}
-	for (uint32_t p = tail + (uint32_t)lane; p < lsize; p += 32u) add(p, dst[p]);
-	uint32_t sa = (uint32_t)(a % 65521u), sb = (uint32_t)(b % 65521u);
-#pragma unroll
-	for (int d = 16; d > 0; d >>= 1) {
-		sa += __shfl_xor_sync(FULL, sa, d);
-		sb += __shfl_xor_sync(FULL, sb, d);
-		sa %= 65521u; sb %= 65521u;
-	}
-	sa = (sa + 1u) % 65521u;
-	sb = (uint32_t)((sb + (uint64_t)lsize) % 65521u);
-	return ((sb << 16) | sa) == want ? MTZ_OK : MTZ_ECODEC;
+	return warp_adler32(dst, lsize, lane) == want ? MTZ_OK : MTZ_ECODEC;
 }
 
 // One warp per job (grid-stride) of a record whose drr_compressiontype is gzip-1 .. gzip-9: the zlib

@@ -20,6 +20,7 @@
 #include "kernels_sha512.cuh"
 #include "kernels_frames.cuh"
 #include "kernels_inflate.cuh"
+#include "kernels_deflate.cuh"
 
 namespace mtz {
 
@@ -55,6 +56,8 @@ struct CodecBufs {
 	uint64_t *vals = nullptr, *offs = nullptr, *out_offs = nullptr;
 	mtz_job *dec = nullptr, *enc = nullptr;
 	mtz_job *dec_gz = nullptr;                          // DECOMPRESS with MTZ_FLAG_GZIP_WIRE: k_inflate's jobs (k_plan_jobs)
+	mtz_job *gz = nullptr;                              // COMPRESS with MTZ_FLAG_GZIP_ENCODE: k_deflate_from_lz4's verdicts
+	uint8_t *d_gz = nullptr;                            // ... and its zlib frames, at d_enc's slot offsets
 	mtz_rec *out_recs = nullptr;
 	RecSums *osums = nullptr;
 	StampStep *steps = nullptr;                         // per-record transitions of the stamp chain
@@ -130,6 +133,8 @@ struct mtz_handle {
 	int device = 0;
 	int sm_count = 0;
 	uint32_t *k_hc_tab = nullptr;      // mtz_k_lz4hc_encode's hash tables (allocated on first use)
+	uint8_t *k_gz_lz = nullptr;        // mtz_k_gzip_encode's LZ4 frames (grown on use)
+	size_t k_gz_lz_cap = 0;
 	std::string err;
 	std::mutex err_mu;
 	std::atomic<int32_t> failed{0};

@@ -318,6 +318,11 @@ int32_t mtz_open(const mtz_config *cfg, mtz_handle **out)
 		return fail(nullptr, MTZ_EINVAL, "GZIP_WIRE forwards the gzip records GZIP_IN inflates: set one of them");
 	if ((full.flags & MTZ_FLAG_GZIP_WIRE) && full.mode == MTZ_MODE_COMPRESS && !(full.flags & MTZ_FLAG_COMPRESSED_IN))
 		return fail(nullptr, MTZ_EINVAL, "COMPRESS: GZIP_WIRE extends COMPRESSED_IN: it needs COMPRESSED_IN");
+	if ((full.flags & MTZ_FLAG_GZIP_ENCODE) && (full.flags & MTZ_FLAG_LZ4_HC))
+		return fail(nullptr, MTZ_EINVAL, "GZIP_ENCODE re-codes K3's parse and LZ4_HC replaces K3: set one of them");
+	if ((full.flags & MTZ_FLAG_GZIP_ENCODE) && (full.flags & MTZ_FLAG_GZIP_IN))
+		return fail(nullptr, MTZ_EINVAL, "GZIP_ENCODE with gzip input: forward the gzip records with GZIP_WIRE "
+		    "instead of GZIP_IN");
 	const cudaDeviceProp &prop = props[0];
 
 	mtz_handle *h = new (std::nothrow) mtz_handle();
@@ -421,6 +426,7 @@ int32_t mtz_close(mtz_handle *h)
 	}
 	codec_free(h->dv_cb);
 	if (h->k_hc_tab) cudaFree(h->k_hc_tab);
+	if (h->k_gz_lz) cudaFree(h->k_gz_lz);
 	if (h->st_post) cudaStreamDestroy(h->st_post);
 	if (h->st_dec) cudaStreamDestroy(h->st_dec);
 	for (int i = 0; i < 2; i++) {
@@ -822,6 +828,13 @@ static bool gzwire_on(const mtz_handle *h)
 	return (cin_on(h) || h->cfg.mode == MTZ_MODE_DECOMPRESS) && (h->cfg.flags & MTZ_FLAG_GZIP_WIRE) != 0;
 }
 
+// COMPRESS with MTZ_FLAG_GZIP_ENCODE re-codes every LZ4 frame K3 makes as a zlib frame
+// (k_deflate_from_lz4) and sends the smaller; the other modes accept the flag and do not change
+static bool gzenc_on(const mtz_handle *h)
+{
+	return h->cfg.mode == MTZ_MODE_COMPRESS && (h->cfg.flags & MTZ_FLAG_GZIP_ENCODE) != 0;
+}
+
 // K3h's hash tables: one per warp of its persistent grid (launch_k3h)
 static size_t hc_tab_bytes(const mtz_handle *h)
 {
@@ -844,6 +857,10 @@ static int32_t codec_alloc(mtz_handle *h, CodecBufs &cb, size_t rec_cap, size_t 
 	if (h->cfg.mode == MTZ_MODE_DECOMPRESS || h->cfg.mode == MTZ_MODE_RECOMPRESS || cin_on(h))
 		MTZ_CU(h, cudaMalloc(&cb.d_logical, scratch_cap + 512));
 	if (h->cfg.mode != MTZ_MODE_DECOMPRESS) MTZ_CU(h, cudaMalloc(&cb.d_enc, scratch_cap + 512));
+	if (gzenc_on(h)) {
+		MTZ_CU(h, cudaMalloc(&cb.gz, rec_cap * sizeof(mtz_job)));
+		MTZ_CU(h, cudaMalloc(&cb.d_gz, scratch_cap + 512));
+	}
 	if (h->cfg.mode == MTZ_MODE_VERIFY && block_lzjb_on(h) && (h->cfg.flags & MTZ_FLAG_BLOCK_FRAMES))
 		MTZ_CU(h, cudaMalloc(&cb.k3_skip, rec_cap * sizeof(uint32_t)));
 	if (lz4hc_on(h)) MTZ_CU(h, cudaMalloc(&cb.hc_tab, hc_tab_bytes(h)));
@@ -875,6 +892,7 @@ static void codec_free(CodecBufs &cb)
 	cudaFree(cb.d_logical); cudaFree(cb.d_enc); cudaFree(cb.d_cres); cudaFree(cb.d_ores);
 	cudaFree(cb.d_outpos); cudaFree(cb.seq_n); cudaFree(cb.cert); cudaFree(cb.k3_skip); cudaFree(cb.hc_tab);
 	cudaFree(cb.chk); cudaFree(cb.chk_sums); cudaFree(cb.d_chk); cudaFree(cb.chk_pos);
+	cudaFree(cb.gz); cudaFree(cb.d_gz);
 	if (cb.h_cres) cudaFreeHost(cb.h_cres);
 	if (cb.h_ores) cudaFreeHost(cb.h_ores);
 	cb = CodecBufs();
@@ -964,7 +982,13 @@ static int32_t codec_launch_dec(mtz_handle *h, cudaStream_t st, CodecBufs &cb, c
 	return MTZ_OK;
 }
 
-// K3 (encode) of one (sub-)batch
+// the grid of k_deflate_from_lz4 over n jobs
+static unsigned defl_grid(const mtz_handle *h, size_t n)
+{
+	return (unsigned)std::max<size_t>(1, std::min<size_t>((n + DEFL_WARPS - 1) / DEFL_WARPS, (size_t)h->sm_count * 8));
+}
+
+// K3 (encode) of one (sub-)batch, and with MTZ_FLAG_GZIP_ENCODE the deflate re-coding of its frames
 // With `st_k3` (and both events) the encoder runs on that low-priority side stream, forked from
 // and joined back into `st`, so that the rest of this slot's work keeps `st`'s high priority.
 static int32_t codec_launch_enc(mtz_handle *h, cudaStream_t st, CodecBufs &cb, size_t nrec, bool compact,
@@ -980,6 +1004,13 @@ static int32_t codec_launch_enc(mtz_handle *h, cudaStream_t st, CodecBufs &cb, s
 	} else {
 		if (cb.cert != nullptr) rc = launch_k3c(h, st_k3, cb, (uint32_t)nrec, compact);
 		if (rc == MTZ_OK) rc = launch_k3(h, st_k3, nullptr, nullptr, cb.enc, (uint32_t)nrec, compact, cb.cert);
+		if (rc == MTZ_OK && cb.gz != nullptr) {
+			// frames at d_enc + slot are re-coded into d_gz + slot: gz_base moves a d_enc address there
+			k_deflate_from_lz4<<<defl_grid(h, nrec), DEFL_THREADS, 0, st_k3>>>(cb.enc, cb.gz, (uint32_t)nrec, 0ull, 0ull,
+			    (uint64_t)(uintptr_t)cb.d_gz - (uint64_t)(uintptr_t)cb.d_enc, true);
+			if (cudaGetLastError() != cudaSuccess) rc = fail(h, MTZ_ECUDA, "k_deflate_from_lz4 launch");
+			else count_launch(h, 1);
+		}
 	}
 	if (rc == MTZ_OK && kb) MTZ_CU(h, cudaEventRecord(kb, st_k3));
 	if (rc == MTZ_OK && st_k3 != st) MTZ_CU(h, cudaStreamWaitEvent(st, kb, 0));
@@ -1004,11 +1035,11 @@ static int32_t codec_launch_post(mtz_handle *h, cudaStream_t st, CodecBufs &cb, 
 	RecSums *osums = all_osums ? all_osums + rec_base : cb.osums;
 	const uint32_t n = (uint32_t)nrec, mode = h->cfg.mode;
 	const unsigned tb = 256, gb = (n + tb - 1) / tb;
-	k_layout<<<gb, tb, 0, st>>>(d_recs, n, cb.cr, cb.dec, cb.enc, cb.vals, cb.d_cres, rec_base, cb.cert, cb.dec_gz);
+	k_layout<<<gb, tb, 0, st>>>(d_recs, n, cb.cr, cb.dec, cb.enc, cb.vals, cb.d_cres, rec_base, cb.cert, cb.dec_gz, cb.gz);
 	k_xscan_u64<<<1, XSCAN_THREADS, 0, st>>>(cb.vals, cb.out_offs, n, cb.d_outpos, cb.d_outpos);
 	const unsigned ga = (unsigned)std::min<size_t>((n + 7) / 8, (size_t)h->sm_count * 8);
 	k_assemble<<<ga, ASM_THREADS, 0, st>>>(d_in, d_recs, n, mode, cb.cr, cb.out_offs, cb.enc,
-	    cb.d_logical, cb.d_enc, d_out, orecs, cb.cert);
+	    cb.d_logical, cb.d_enc, d_out, orecs, cb.cert, cb.gz);
 	MTZ_CU(h, cudaGetLastError());
 	// output records of a codec batch are smaller than the logical size: decide by the input's
 	launch_k1_kernel(h, st, d_out, orecs, n, osums, 312u, cb.avg_out_rec);
@@ -1517,6 +1548,7 @@ static int32_t dev_finish_impl(mtz_handle *h, const uint64_t carry_in[4], const 
 		h->cstats.zle_decoded += c.n_zle;
 		h->cstats.gzip_decoded += c.n_gzip;
 		h->cstats.gzip_passed += c.n_gzpass;
+		h->cstats.gzip_encoded += c.n_gz_enc;
 	}
 	if (out_bytes) *out_bytes = ob;
 	rc = account_result(h, r, h->dv_first, h->dv_nrec, h->dv_in_bytes, ob, block_on(h) ? &h->bpend : nullptr);
@@ -1623,7 +1655,7 @@ static int32_t batch_accept(mtz_handle *h, const Slot &s, BatchCut &bc, const ui
 			// the lz4-stage-v1 wire puts a preamble in front of every BEGIN: BEGIN opens its batch
 			if (bc.cnt > 0) return 0;
 			bc.emit_pre = true;
-			bc.pre_flags = wire_orig_lz4(feat) | (gzwire_on(h) ? WIRE_F_GZIP : 0u);
+			bc.pre_flags = wire_orig_lz4(feat) | (gzwire_on(h) || gzenc_on(h) ? WIRE_F_GZIP : 0u);
 		} else if (h->cfg.mode == MTZ_MODE_DECOMPRESS) {
 			if (!ws->pre_seen)
 				return fail(h, MTZ_EINVAL, "DECOMPRESS: stream was not produced by the COMPRESS stage");
@@ -1697,6 +1729,7 @@ static int32_t harvest(mtz_handle *h, Slot &s)
 		h->cstats.zle_decoded += c.n_zle;
 		h->cstats.gzip_decoded += c.n_gzip;
 		h->cstats.gzip_passed += c.n_gzpass;
+		h->cstats.gzip_encoded += c.n_gz_enc;
 	}
 	int32_t rc = account_result(h, *s.h_res, s.first_rec, s.nrec, s.bytes, s.out_bytes,
 	    block_on(h) ? &bp : nullptr);
@@ -2065,6 +2098,40 @@ int32_t mtz_k_lz4_encode(mtz_handle *h, const void *d_src, void *d_dst, mtz_job 
 	// MTZ_K3_FORCE_COMPACT: the caller vouches that every job is a 128 KiB-class block (experiments)
 	const char *e = getenv("MTZ_K3_FORCE_COMPACT");
 	return launch_k3(h, st, d_src, d_dst, d_jobs, njobs, e != nullptr && atoi(e) != 0);
+}
+
+// K3, then k_deflate_from_lz4 on the same stream: K3's frames go to a scratch of the handle at the jobs'
+// dst_off, the zlib frames to d_dst.  Reads the job table to size that scratch, so it synchronises.
+int32_t mtz_k_gzip_encode(mtz_handle *h, const void *d_src, void *d_dst, mtz_job *d_jobs,
+    uint32_t njobs, void *cuda_stream)
+{
+	CHECK_H(h);
+	if (njobs == 0) return MTZ_OK;
+	if (((uintptr_t)d_dst & 3u) != 0) return fail(h, MTZ_EINVAL, "mtz_k_gzip_encode: d_dst must be 4-byte aligned");
+	MTZ_CU(h, cudaSetDevice(h->device));
+	cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : h->st;
+	std::vector<mtz_job> jobs(njobs);
+	MTZ_CU(h, cudaMemcpyAsync(jobs.data(), d_jobs, njobs * sizeof(mtz_job), cudaMemcpyDeviceToHost, st));
+	MTZ_CU(h, cudaStreamSynchronize(st));
+	size_t need = 0;
+	for (const mtz_job &j : jobs) {
+		if (j.lsize == 0) continue;
+		if ((j.dst_off & 3u) != 0) return fail(h, MTZ_EINVAL, "mtz_k_gzip_encode: every dst_off must be 4-byte aligned");
+		need = std::max<size_t>(need, (size_t)j.dst_off + j.lsize);
+	}
+	if (need > h->k_gz_lz_cap) {
+		if (h->k_gz_lz) MTZ_CU(h, cudaFree(h->k_gz_lz));
+		h->k_gz_lz = nullptr; h->k_gz_lz_cap = 0;
+		MTZ_CU(h, cudaMalloc(&h->k_gz_lz, need + 16));
+		h->k_gz_lz_cap = need;
+	}
+	int32_t rc = launch_k3(h, st, d_src, h->k_gz_lz, d_jobs, njobs, false);
+	if (rc != MTZ_OK) return rc;
+	k_deflate_from_lz4<<<defl_grid(h, njobs), DEFL_THREADS, 0, st>>>(d_jobs, d_jobs, njobs, (uint64_t)(uintptr_t)d_src,
+	    (uint64_t)(uintptr_t)h->k_gz_lz, (uint64_t)(uintptr_t)d_dst, false);
+	MTZ_CU(h, cudaGetLastError());
+	count_launch(h, 1);
+	return MTZ_OK;
 }
 
 // K3h over njobs jobs with `tabs` (hc_tab_bytes): the persistent grid has exactly the warps the

@@ -116,16 +116,18 @@ class BackupSender(object):
         stage off the job object is left exactly as the reference has it (no `wire` field).
         On the stage wire with gpu.sendCompressed, `wireGzip` says whether gzip records travel as
         their disk frames (MTZ_FLAG_GZIP_WIRE): only when every requester also advertised
-        `acceptGzip: true`, since the receiver's stage then inflates them."""
+        `acceptGzip: true`, since the receiver's stage then inflates them.  With gpu.gzipEncode the
+        same condition, with or without gpu.sendCompressed, also makes COMPRESS deflate the records it
+        encodes (MTZ_FLAG_GZIP_ENCODE)."""
         if not self._gpu or self._gpu.get("mode", "off") == "off":
             return
         compress = self._gpu["mode"] == "compress" and \
             all(j.get("accept") == "lz4-stage-v1" for j in jobs)
-        gzip_wire = compress and bool(self._gpu.get("sendCompressed")) and \
-            all(j.get("acceptGzip") is True for j in jobs)
+        gzip_capable = bool(self._gpu.get("sendCompressed") or self._gpu.get("gzipEncode"))
+        gzip_wire = compress and gzip_capable and all(j.get("acceptGzip") is True for j in jobs)
         for j in jobs:
             j["wire"] = "lz4-stage-v1" if compress else "raw"
-            if compress and self._gpu.get("sendCompressed"):
+            if compress and gzip_capable:
                 j["wireGzip"] = gzip_wire
 
     def _send_compressed(self, backupJob):
@@ -153,16 +155,19 @@ class BackupSender(object):
                                 compressed_input=self._send_compressed(backupJob),
                                 gzip_input=self._send_compressed(backupJob) and bool(g.get("sendGzip"))
                                 and not backupJob.get("wireGzip"),
-                                gzip_wire=self._send_compressed(backupJob) and bool(backupJob.get("wireGzip")))
+                                gzip_wire=self._send_compressed(backupJob) and bool(backupJob.get("wireGzip")),
+                                gzip_encode=g["mode"] == "compress" and bool(g.get("gzipEncode"))
+                                and bool(backupJob.get("wireGzip")))
 
     def _stage_stats(self, stage):
         """job.gpu: the stage counters, plus `blocks` (block-checksum counters) with
         gpu.blockChecksums set and `compressed_in` (mtz_get_compressed_in_stats) with gpu.sendCompressed,
-        gzip_decoded included with gpu.sendGzip, gzip_passed on a `wireGzip` job"""
+        gzip_decoded included with gpu.sendGzip, gzip_passed on a `wireGzip` job; with gpu.gzipEncode
+        `compressed_in` too, gzip_encoded included on a `wireGzip` job"""
         st = stage.stats()
         if self._gpu.get("blockChecksums"):
             st["blocks"] = stage.block_stats()
-        if self._gpu.get("sendCompressed"):
+        if self._gpu.get("sendCompressed") or self._gpu.get("gzipEncode"):
             st["compressed_in"] = stage.compressed_in_stats()
         return st
 

@@ -22,7 +22,7 @@ class GpuSnapshotStage(object):
     def __init__(self, mode="verify", device=0, ring_bytes=0, batch_bytes=0, n_slots=0,
                  out_ring_bytes=0, flags=0, devices=None, block_checksums=False, block_sha256=False,
                  block_sha512=False, block_frames=False, block_lzjb=False, block_logical=False,
-                 lz4_hc=False, compressed_input=False, gzip_input=False, gzip_wire=False):
+                 lz4_hc=False, compressed_input=False, gzip_input=False, gzip_wire=False, gzip_encode=False):
         """``devices`` = CUDA ordinals of a device group: the GPUs of one box run as ONE stage,
         batch b of the stream on ``devices[b % len(devices)]`` (mtz_config.devices[]).
         ``block_checksums`` = MTZ_FLAG_BLOCK_CKSUM: every DRR_WRITE is also checked against the
@@ -64,7 +64,12 @@ class GpuSnapshotStage(object):
         reports ``gzip_passed``).  DECOMPRESS accepts that bit, inflates the gzip records on the GPU by
         ``gzip_input``'s rule and writes them raw, as plain `zfs send` would have (``gzip_decoded``); a
         DECOMPRESS stage without it refuses such a wire with EFORMAT.  The other modes accept it and do
-        not change."""
+        not change.
+        ``gzip_encode`` = MTZ_FLAG_GZIP_ENCODE, never with ``lz4_hc`` or ``gzip_input``: COMPRESS also re-codes
+        each LZ4 frame it makes as a zlib frame and sends a record as gzip-1 when that is smaller; every
+        preamble carries the gzip capability bit, so the receiver needs ``gzip_wire``.
+        ``compressed_in_stats()`` then also reports ``gzip_encoded``.  The other modes accept it and do not
+        change."""
         if block_checksums:
             flags |= N.FLAG_BLOCK_CKSUM
         if block_sha256:
@@ -87,6 +92,9 @@ class GpuSnapshotStage(object):
             flags |= N.FLAG_GZIP_WIRE
         self._gzip_input = bool(gzip_input)
         self._gzip_wire = bool(gzip_wire)
+        if gzip_encode:
+            flags |= N.FLAG_GZIP_ENCODE
+        self._gzip_encode = bool(gzip_encode)
         self._L = N.lib()
         self._h = C.c_void_p()
         cfg = N.Config()
@@ -161,6 +169,8 @@ class GpuSnapshotStage(object):
             del d["gzip_decoded"]
         if not self._gzip_wire:
             del d["gzip_passed"]
+        if not self._gzip_encode:
+            del d["gzip_encoded"]
         return d
 
     def end_checksum(self):

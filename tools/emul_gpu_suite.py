@@ -55,6 +55,7 @@ PARAMS = {
     "test_inflated_output_equals_the_model": [("gzip-1", 8192), ("gzip-6", 8192), ("gzip-9", 8192), ("mixed", 8192)],
     "test_gzip_block_counters": [(False, False), (True, True)],
     "test_round_trip_equals_the_model": [("gzip-1", 8192), ("gzip-6", 8192), ("gzip-9", 8192), ("mixed", 8192)],
+    "test_compress_equals_the_model": [("pgpage", 131072), ("mixed", 8192)],
 }
 SKIP = {"test_sixteen_mib_record": "16 MiB blocks take minutes per encode on the emulator",
         "test_size_independent_properties_at_2gib": "2 GiB of LZ4 work is out of reach for the emulator",
@@ -64,6 +65,8 @@ SKIP = {"test_sixteen_mib_record": "16 MiB blocks take minutes per encode on the
                                       "on host memory",
         "test_device_group": "needs two GPUs",
         "test_fanout_of_two_peers": "needs two GPUs",
+        "test_kernel_equals_the_model": "its device buffers are torch tensors; tests/test_emul_gzip_encode.py runs "
+                                        "mtz_k_gzip_encode on host memory",
         "test_kernel_equals_the_oracle_on_thousands_of_jobs": "3000 jobs and a 16 MiB block take hours on the emulator; "
                                                               "tests/test_emul_lz4hc.py runs K3h inside guard pages",
         "test_host_pipeline_compress_hc_to_a_plain_decompress": "needs the fake-zfs fixture (pytest)",
@@ -90,12 +93,13 @@ def main():
     import test_gpu_compressed_in as CI
     import test_gpu_gzip_in as GZ
     import test_gpu_gzip_wire as GW
+    import test_gpu_gzip_encode as GE
     import test_gpu_lz4 as Z
     import test_gpu_lz4hc as HC
     import test_gpu_stream as S
     import test_gpu_verify as V
     tot = fail = 0
-    for mod in (V, S, Z, K, B, H, W, F, J, L, HC, CI, GZ, GW):
+    for mod in (V, S, Z, K, B, H, W, F, J, L, HC, CI, GZ, GW, GE):
         for name, fn in inspect.getmembers(mod, inspect.isfunction):
             if not name.startswith("test_") or filt not in name:
                 continue

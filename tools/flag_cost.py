@@ -36,6 +36,11 @@ power limit and max SM clock the numbers were taken on.
                  against DECOMPRESS with gzip_wire of the gzip wire, and DECOMPRESS with gzip_wire of today's
                  wire (no gzip record on it): resident step, mtz_process_host, k_inflate and K2 device time;
                  every DECOMPRESS output is checked against plain(x); --pools picks some of the pools
+  gzip_encode    MTZ_FLAG_GZIP_ENCODE: COMPRESS against COMPRESS with gzip_encode of pg-page 128 KiB records,
+                 raw and (--mixed-gib of them) as a `send -c` stream of block_ref.mixed_codecs with
+                 compressed_input: wire bytes, resident step with K3's and k_deflate_from_lz4's device time,
+                 mtz_process_host, the ring API through a pipe, and the receiver's DECOMPRESS (with
+                 gzip_wire on the new wire) with k_inflate's and K2's device time
 
 A resident step is timed with CUDA events around dev_submit + dev_finish on a side stream, a host pass
 with the host clock around mtz_process_host; kernel device times come from torch.profiler in a pass of
@@ -639,6 +644,44 @@ def gzip_wire(a):
     return res
 
 
+def gzip_encode(a):
+    """MTZ_FLAG_GZIP_ENCODE (module docstring): a raw pg-page stream, and a `send -c` stream of the
+    block_ref.mixed_codecs pool with compressed_input"""
+    import numpy as np
+    import bench
+    import gzip_encode_ref as GE
+    from manatee_b200 import GpuSnapshotStage, index_host
+    res = {"payload": "pg-page 128 KiB records (oracle.gen_payload(PAYLOAD_PGPAGE, r, 131072))"}
+    p = synth(a.gib, O.PAYLOAD_PGPAGE)
+    m = synth(a.mixed_gib, O.PAYLOAD_PGPAGE)
+    for sname, x, kw in (("pgpage", p, {}), ("mixed_codecs_send_c", CI.send_c(O, m, 9, R.mixed_codecs),
+                                            {"compressed_input": True})):
+        logical = int(index_host(CI.plain(O, x) if kw else x)[0]["lsize"].sum())
+        r = {"logical_bytes": logical, "input_bytes": int(x.size)}
+        send = {"lz4_wire": ("compress", kw, x), "gzip_encode": ("compress", dict(kw, gzip_encode=True), x)}
+        r["sender_resident"], _ = dev_legs(a, send, logical, "gzip_encode", ("k3_lz4_encode", "k_deflate_from_lz4"))
+        r["sender_host"], wires = host_legs(a, send, logical)
+        r["lz4_wire_bytes"], r["gzip_wire_bytes"] = int(wires["lz4_wire"].size), int(wires["gzip_encode"].size)
+        r["wire_saving_pct"] = 100.0 * (1 - r["gzip_wire_bytes"] / r["lz4_wire_bytes"])
+        r["wire_records_lz4_gzip"] = GE.counts(O, wires["gzip_encode"])
+        secs = {n: [] for n in send}
+        for _, n in alternate(send, a.ring_steps):
+            with GpuSnapshotStage("compress", **send[n][1]) as g:
+                dt, ok, detail = bench.ring_run(g, x, producer="pipe")
+                assert ok, detail
+                secs[n].append(dt)
+        r["sender_ring_pipe"] = {n + "_logical_gbps_mean": logical / (sum(v) / len(v)) / 1e9 for n, v in secs.items()}
+        lzw, gzw = wires["lz4_wire"], wires["gzip_encode"]
+        want = CI.plain(O, x) if kw else x
+        recv = {"lz4_wire": ("decompress", {}, O.wire_strip(lzw)),
+                "gzip_encode": ("decompress", {"gzip_wire": True}, O.wire_strip(gzw))}
+        r["receiver_resident"], outs = dev_legs(a, recv, logical, "gzip_encode", ("k_inflate", "k2_lz4_decode"))
+        r["resident_decompressed_equals_input"] = {n: bool(np.array_equal(outs[n], want)) for n in recv}
+        res[sname] = r
+        del x, wires, outs
+    return res
+
+
 SHA_OPTIONS = dict(verify_gib=16.0, host_gib=2.0, recompress_gib=1.0, steps=10, warmup=2, host_steps=4,
                    profile_steps=3)
 FRAME_OPTIONS = dict(verify_gib=16.0, host_gib=2.0, ring_gib=8.0, steps=10, warmup=2, host_steps=4, ring_steps=3,
@@ -657,6 +700,7 @@ WORKLOADS = {
     "gzip_in": (gzip_in, dict(gib=0.5, steps=5, warmup=1, host_steps=3, ring_steps=3, profile_steps=2)),
     "gzip_wire": (gzip_wire, dict(gib=0.5, steps=5, warmup=1, host_steps=3, ring_steps=3, profile_steps=2,
                                   pools=",".join(s[0] for s in GZIP_STREAMS))),
+    "gzip_encode": (gzip_encode, dict(gib=0.5, mixed_gib=0.125, steps=5, warmup=1, host_steps=3, ring_steps=3, profile_steps=2)),
 }
 
 
